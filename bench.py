@@ -31,6 +31,11 @@ sys.path.insert(0, str(ROOT))
 
 METRIC = "training scenes/sec (20k-pt SUN-RGBD synth, 256 queries)"
 UNIT = "scenes/s"
+# NVIDIA H100 SXM data sheet (700 W card): dense BF16 tensor rate, HBM3 bandwidth.  Used as the roofline peaks when
+# no measured peaks are given; a card with a lower power limit does not reach them.
+H100_BF16_TFLOPS = 989.0
+H100_HBM_GBS = 3350.0
+DUMP_SAMPLE = 1 << 20     # parameter / gradient entries kept by --dump-outputs (fixed seeded sample)
 
 
 def parse():
@@ -48,6 +53,9 @@ def parse():
     p.add_argument("--nsplit", type=int, default=3, help="bf16 planes per fp32 operand on the tensor-core path")
     p.add_argument("--num-classes", type=int, default=46, help="text rows (46: SUN RGB-D prompts; 232: ScanNet-200 set)")
     p.add_argument("--image", default="531x730", help="image height x width (ScanNet shape: 968x1296)")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="write what the last timed step computed (loss, loss terms, a fixed sample of the updated "
+                        "parameters and of their gradients) as DIR/<name>.npy")
     return p.parse_args()
 
 
@@ -64,7 +72,7 @@ def workload_config(a, world):
             "global_batch": a.batch_per_gpu * world, "parallelism": f"dp{world}",
             "weights": "random-init (no checkpoints offline)", "num_text_classes": a.num_classes,
             "image_hw": [h, w],
-            "l2": "per-step working set (~2 GB of SA / attention activations) >> 126 MB L2; inputs differ per step"}
+            "l2": "per-step working set (~2 GB of SA / attention activations) >> 50 MB L2; inputs differ per step"}
 
 
 # --------------------------------------------------------------------------- clocks
@@ -178,14 +186,14 @@ def attention_roofline(a, device):
     4 * B * H * Lq * Lk * hd per launch (QK^T + PV)."""
     import ctypes
 
-    from coda_neurips2023_b200 import _lib, attention_sm100
+    from coda_neurips2023_b200 import _lib
 
     peaks = {}
     try:
         peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())
     except OSError:
         pass
-    peak = float(peaks.get("bf16_tflops", 1590.0))
+    peak = float(peaks.get("bf16_tflops", H100_BF16_TFLOPS))
     b, h, lq, lk, hd = a.batch_per_gpu, 4, 2048, 2048, 64
     q = torch.randn(lq, b, h * hd, device=device)
     k = torch.randn(lk, b, h * hd, device=device)
@@ -222,10 +230,11 @@ def attention_roofline(a, device):
     flops = 4.0 * b * h * lq * lk * hd          # algorithmic: QK^T + PV, 2 flops per MAC
     achieved = flops / (ms * 1e-3) / 1e12
     nprod = {1: 1.0, 2: 3.0, 3: 5.5}[ns]       # QK^T: 1 / 3 / 6 plane products, PV: 1 / 3 / 5 (P carries 2 planes)
-    return {"bound": "tensor", "kernel": "attn_fwd_kernel<64,%d> (tcgen05 fused encoder self-attention forward, "
+    return {"bound": "tensor", "kernel": "attn_fwd_kernel<64,%d> (wgmma fused encoder self-attention forward, "
             "L=2048, 4 heads x 64, batch %d)" % (ns, b),
             "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-            "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst; kernel timed alone)" if peaks else "fallback 1590",
+            "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst; kernel timed alone)" if peaks
+            else "H100 SXM data sheet, dense BF16",
             "flops_per_launch": flops, "ms_per_launch": ms, "traffic": None,
             "tensor_pipe_flops_per_launch": flops * nprod,
             "tensor_pipe_frac": achieved * nprod / peak,
@@ -260,15 +269,15 @@ def _peaks():
 
 
 def sa_wgrad_roofline(a, device):
-    """The dominant kernel by share of the step (profiles/r02_step_kernels.txt: gemm_tn32_kernel<128>, every weight
-    gradient of the step, 11 %), timed alone on its longest launch: the weight gradient of the third set-abstraction
+    """The weight-gradient kernel (gemm_tn32_kernel<128>, every weight gradient of the step), timed alone on its
+    longest launch: the weight gradient of the third set-abstraction
     layer, dW2 (256 x 128) = dY2^T A2 over R = B * 2048 * 64 rows, with the step's prologues (dY2 from the pre-BN
     activation y2 + the max-pooled gradient; A2 = relu(bn(y1))).  The kernel streams both fp32 activations once:
     algorithmic bytes = 4 R (256 + 128) (+ 21 MB pooled gradient / arg-max); peak = MEASURED_PEAKS.json hbm_gbs."""
     from coda_neurips2023_b200 import ops
 
     peaks = _peaks()
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
     rows, m, n, group = a.batch_per_gpu * 2048 * 64, 256, 128, 64
     y2 = torch.randn(rows, m, device=device)
     y1 = torch.randn(rows, n, device=device)
@@ -283,15 +292,13 @@ def sa_wgrad_roofline(a, device):
                                             b_scale=sb, b_shift=tb, out=out))
     nbytes = 4.0 * rows * (m + n) + 5.0 * (rows // group) * m + 4.0 * m * n
     achieved = nbytes / (ms * 1e-3) / 1e9
-    return {"bound": "hbm", "kernel": "gemm_tn32_kernel<128> (tcgen05 weight-gradient GEMM on fp32 rows, BatchNorm-backward / "
+    return {"bound": "hbm", "kernel": "gemm_tn32_kernel<128> (wgmma weight-gradient GEMM on fp32 rows, BatchNorm-backward / "
             "BatchNorm+ReLU prologues in-kernel; SA layer 3: dW (%d x %d) over %d rows)" % (m, n, rows),
             "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650",
-            "bytes_per_launch": nbytes, "ms_per_launch": ms,
-            "traffic": 1.632e9, "traffic_source": "ncu dram__bytes_read.sum + dram__bytes_write.sum of this launch "
-                                                   "(profiles/r02_sa_mlp_traffic.txt)",
+            "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet, HBM3",
+            "bytes_per_launch": nbytes, "ms_per_launch": ms, "traffic": None,
             "useful_tflops": 2.0 * rows * m * n / (ms * 1e-3) / 1e12,
-            "note": "working set (1.6 GB) >> 126 MB L2: every timed launch streams from HBM"}
+            "note": "working set (1.6 GB) >> 50 MB L2: every timed launch streams from HBM"}
 
 
 def sa_forward_roofline(a, device):
@@ -301,7 +308,7 @@ def sa_forward_roofline(a, device):
     from coda_neurips2023_b200 import ops
 
     peaks = _peaks()
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
     rows, k, n, ns = a.batch_per_gpu * 2048 * 64, 128, 256, a.nsplit
     y1 = torch.randn(rows, k, device=device)
     wp = ops.pack_split(torch.randn(n, k, device=device) / k ** 0.5, n, k, k, 1, 3)
@@ -311,12 +318,11 @@ def sa_forward_roofline(a, device):
                                            want_stats=True, nsplit=ns))
     nbytes = 4.0 * rows * (k + n) + 2.0 * ns * n * k
     achieved = nbytes / (ms * 1e-3) / 1e9
-    return {"bound": "hbm", "kernel": "gemm_a32_kernel<%d,128> (tcgen05 GEMM, fp32 A split in-kernel into TMEM, BN+ReLU "
-            "prologue, BN-statistics epilogue; SA layer 3 forward: %d x %d x %d)" % (ns, rows, n, k),
+    return {"bound": "hbm", "kernel": "gemm_a32_kernel<%d,128> (wgmma GEMM, fp32 A split in-kernel into register "
+            "fragments, BN+ReLU prologue, BN-statistics epilogue; SA layer 3 forward: %d x %d x %d)" % (ns, rows, n, k),
             "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650",
-            "bytes_per_launch": nbytes, "ms_per_launch": ms, "traffic": 1.549e9,
-            "traffic_source": "ncu dram bytes of this launch (profiles/r02_sa_mlp_traffic.txt)",
+            "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet, HBM3",
+            "bytes_per_launch": nbytes, "ms_per_launch": ms, "traffic": None,
             "useful_tflops": 2.0 * rows * n * k / (ms * 1e-3) / 1e12,
             "tensor_pipe_tflops": 2.0 * rows * n * k * {2: 3, 3: 6}[ns] / (ms * 1e-3) / 1e12}
 
@@ -395,10 +401,12 @@ def run_ours(a):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for i in range(a.steps):
-        loss, _ = step(resident[i % nb], 0.0)
+        loss, loss_terms = step(resident[i % nb], 0.0)
     e1.record()
     barrier()
     launches = (_lib.LAUNCHES - launches0) if not use_graph else step.launches_per_step * a.steps
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, loss, loss_terms, step.flat)
     ms_dev = max_over_ranks(e0.elapsed_time(e1))
     assert torch.isfinite(loss).item(), "non-finite loss"
     # ---------------- end-to-end leg (host buffers, H2D + loss read-back inside) ----------------
@@ -452,6 +460,25 @@ def run_ours(a):
                                           "C restatement of its CUDA-only ops; use --impl reference for more steps"}
     _emit(line)
     _finish(world, device)
+
+
+def dump_outputs(out_dir, loss, loss_terms, flat):
+    """What the last timed step computed, as float32 / float64 .npy files: the loss, every scalar loss term, and the
+    same seeded sample of the updated parameters and of their gradients (the full vectors are larger than needed
+    to compare two builds)."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    np.save(d / "loss.npy", np.array([float(loss)], dtype=np.float64))
+    for k, v in sorted(loss_terms.items()):
+        if isinstance(v, torch.Tensor) and v.numel() == 1:
+            np.save(d / f"loss_term.{k}.npy", np.array([float(v.detach())], dtype=np.float64))
+    total = flat.flat_param.numel()
+    gen = np.random.default_rng(0)
+    idx = np.sort(gen.choice(total, size=min(DUMP_SAMPLE, total), replace=False))
+    sel = torch.from_numpy(idx).to(flat.flat_param.device)
+    np.save(d / "param_sample_index.npy", idx.astype(np.float64))
+    np.save(d / "param_sample.npy", flat.flat_param.detach()[sel].float().cpu().numpy())
+    np.save(d / "grad_sample.npy", flat.flat_grad.detach()[sel].float().cpu().numpy())
 
 
 def _finish(world, device):

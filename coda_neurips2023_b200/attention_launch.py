@@ -1,4 +1,4 @@
-"""Launchers of the tcgen05 attention forward and backward (include/coda_attention.h) and the
+"""Launchers of the wgmma attention forward and backward (include/coda_attention.h) and the
 torch-side twin of their counter-based dropout mask (used by the tests to build the same mask)."""
 from __future__ import annotations
 
@@ -75,10 +75,9 @@ def radius_mask_bits(xyz: torch.Tensor, radius: float):
 
 
 # operand planes of q / k / v in the forward of the fp32 attention: 2 = 16 mantissa bits, three cross products per
-# contraction (3 = 24 bits, six).  Measured against the reference goldens on the B200 (tests/test_model_gpu.py, all
-# seven cases incl. the BASELINE-size and ScanNet-size ones): the forward's worst deviation is THE SAME with 2 and 3
-# planes (2.9e-5 / 4.2e-5 at full size, <= 5.2e-5 at the small sizes; bar 1e-4) -- the attention operands are not what
-# limits parity -- so the step runs on 2.  CODA_ATTN_NSPLIT=3 restores the wider split.
+# contraction (3 = 24 bits, six).  Against the reference goldens (tests/test_model_gpu.py, all seven cases incl. the
+# BASELINE-size and ScanNet-size ones) the forward's worst deviation does not change between 2 and 3 planes -- the
+# attention operands are not what limits parity -- so the step runs on 2.  CODA_ATTN_NSPLIT=3 restores the wider split.
 import os as _os
 FORWARD_NSPLIT = int(_os.environ.get("CODA_ATTN_NSPLIT", "2"))
 
@@ -192,7 +191,7 @@ def dropout_mult(bh: int, lq: int, lk: int, dropout_p: float, salt: int, device)
 
 
 def backward(q, k, v, out, dout, lse, nhead: int, dropout_p: float = 0.0, salt: int = 0, mask=None, grads=None):
-    """Fused tcgen05 backward (head dim 64 / 128): returns (dq, dk, dv), each shaped like its input.  q / k / v may
+    """Fused wgmma backward (head dim 64 / 128): returns (dq, dk, dv), each shaped like its input.  q / k / v may
     be row-strided slices of a fused projection (read in place); `grads` = preallocated (dq, dk, dv) views, e.g. the
     slices of ONE packed gradient buffer of that projection (written in place, nothing to concatenate)."""
     lq, b, e = q.shape

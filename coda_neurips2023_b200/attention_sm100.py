@@ -1,9 +1,9 @@
-"""Fused multi-head attention on tcgen05 tensor cores (include/coda_attention.h).
+"""Fused multi-head attention on wgmma tensor cores (include/coda_attention.h).
 
 forward : one launch per attention call; S = Q K^T, online softmax and O = P V are
-          tiled through TMEM, the (Lq x Lk) probabilities never reach HBM.
-backward: two tcgen05 kernels (dQ; dK / dV) that recompute P tile by tile from the saved
-          log-sum-exp (csrc/attention_bwd_sm100.cu); nothing of size Lq x Lk is stored.
+          tiled through registers, the (Lq x Lk) probabilities never reach HBM.
+backward: two wgmma kernels (dQ; dK / dV) that recompute P tile by tile from the saved
+          log-sum-exp (csrc/attention_bwd_sm90.cu); nothing of size Lq x Lk is stored.
 `_math` below is the plain-tensor formulation used by the tests as the numerics reference and by
 the causal CLIP text tower, which runs once at model construction (never inside the step).
 """
@@ -72,7 +72,7 @@ class _Attention(torch.autograd.Function):
         from . import attention_launch
 
         a, b, c, out, lse = ctx.saved_tensors
-        # fused tcgen05 backward (dQ kernel + dK/dV kernel); P is recomputed tile by tile, never stored
+        # fused wgmma backward (dQ kernel + dK/dV kernel); P is recomputed tile by tile, never stored
         kw = dict(mask=ctx.mask)
         if ctx.layout == "qkv":
             e = a.shape[-1] // 3
@@ -113,7 +113,7 @@ def attention_fused(a, b, layout, nhead, dropout_p=0.0, training=False, mask=Non
         raise RuntimeError("attention: CPU not supported")
     e = a.shape[-1] // (3 if layout == "qkv" else 2)
     if a.dtype != torch.float32 or (e // nhead) not in (64, 128):
-        # head dims the tcgen05 kernels do not cover (reduced test configurations): the three-tensor entry decides
+        # head dims the wgmma kernels do not cover (reduced test configurations): the three-tensor entry decides
         return attention(a[..., :e], a[..., e: 2 * e], a[..., 2 * e:] if layout == "qkv" else b, nhead, dropout_p,
                          training, False, mask)
     from . import attention_launch

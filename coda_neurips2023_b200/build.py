@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA library (sm_100a only) with plain nvcc.
+"""In-tree build of the CUDA library (sm_90a, H100) with plain nvcc.
 
 The product is ONE C-ABI shared library, ``csrc/libcoda_b200.so``; it has no
 torch / pybind dependency, so a full rebuild takes seconds and the same binary
@@ -19,7 +19,7 @@ LIB = CSRC / "libcoda_b200.so"
 OBJ_DIR = CSRC / "build"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",
@@ -47,7 +47,7 @@ def sources():
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every ``csrc/*.cu`` for sm_100a and link ``libcoda_b200.so``."""
+    """Compile every ``csrc/*.cu`` for sm_90a and link ``libcoda_b200.so``."""
     srcs = sources()
     hdrs = sorted(CSRC.glob("*.cuh")) + sorted((CSRC.parent.parent / "include").glob("*.h"))
     stamp = OBJ_DIR / "stamp.txt"

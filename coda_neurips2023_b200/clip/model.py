@@ -25,7 +25,7 @@ from .. import ops
 
 
 def _linear(x, w, b, quick_gelu=False, residual=None):
-    """fp16 activations x fp16 weights on the fp16 tcgen05 path (fp16 written by the epilogue,
+    """fp16 activations x fp16 weights on the fp16 wgmma path (fp16 written by the epilogue,
     QuickGELU and the block's residual connection fused); fp32 (CPU checks, small test models) through torch."""
     if x.is_cuda and x.dtype == torch.float16 and x.shape[-1] % 64 == 0:
         return ops.linear(x, w, b, quick_gelu=quick_gelu, residual=residual)
@@ -72,7 +72,7 @@ class _PackedSelfAttention(nn.Module):
             from .. import attention_launch
             # q / k / v stay fp16 slices of the fused projection: the pack kernel reads them in place
             if x.shape[0] <= 64:
-                # image tower (50 tokens): fused tcgen05 attention on HALF operands, the tensor core's native type
+                # image tower (50 tokens): fused wgmma attention on HALF operands, the tensor core's native type
                 out = attention_launch.forward_half(q, k, v, self.num_heads)
             else:
                 # longer sequences: 2 bf16 planes (16 mantissa bits >= fp16's 11)
@@ -154,7 +154,7 @@ class VisionTransformer(nn.Module):
         return x, all_tokens
 
     def _project(self, x):
-        """x @ proj (reference CLIP/clip/model.py:655-657).  fp16 on the device: the tcgen05 GEMM with the transposed
+        """x @ proj (reference CLIP/clip/model.py:655-657).  fp16 on the device: the wgmma GEMM with the transposed
         projection as its K-major weight (cached; the tower is frozen)."""
         if not (x.is_cuda and x.dtype == torch.float16 and x.shape[-1] % 64 == 0):
             return x @ self.proj

@@ -1,4 +1,4 @@
-"""Hungarian-matched set criterion of CoDA, B200-native.
+"""Hungarian-matched set criterion of CoDA, H100-native.
 
 Mirror of reference criterion.py: `Matcher` (:12-86), `SetCriterion` (:89-1216)
 and `build_criterion` (:1219-1281), same call signatures (`criterion(outputs,

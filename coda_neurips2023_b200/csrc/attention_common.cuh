@@ -1,9 +1,9 @@
-// Shared pieces of the tcgen05 attention kernels (forward: attention_sm100.cu, backward:
-// attention_bwd_sm100.cu): tile sizes, split-product tables, bf16 plane splitting, dropout hash.
+// Shared pieces of the wgmma attention kernels (forward: attention_sm90.cu, backward:
+// attention_bwd_sm90.cu): tile sizes, split-product tables, bf16 plane splitting, dropout hash.
 #pragma once
 #include <math.h>
 
-#include "sm100_primitives.cuh"
+#include "sm90_primitives.cuh"
 
 namespace coda {
 namespace attn {

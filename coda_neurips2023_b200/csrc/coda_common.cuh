@@ -1,4 +1,4 @@
-// Shared device/host helpers for the coda_b200 kernels (sm_100a only).
+// Shared device/host helpers for the coda_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

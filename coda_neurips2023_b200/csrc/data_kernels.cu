@@ -1,4 +1,4 @@
-// Data layer on the device (sm_100a): the per-scene numpy pipeline of the reference's dataset __getitem__
+// Data layer on the device (sm_90a): the per-scene numpy pipeline of the reference's dataset __getitem__
 // (datasets/sunrgbd_anonymous_aligned_image.py:618-795, utils/random_cuboid.py, utils/pc_util.py:24-32) for a whole
 // batch of raw scenes that are already resident in HBM:
 //

@@ -1,5 +1,5 @@
 // Warp-primitive kernels of the 3DETR encoder/decoder and of the matcher for
-// B200 (sm_100a): LayerNorm fwd/bwd, row softmax, fused Fourier positional
+// H100 (sm_90a): LayerNorm fwd/bwd, row softmax, fused Fourier positional
 // encoding, generalised 3-D IoU with rotated-rectangle clipping, and a
 // warp-per-scene Hungarian solver.  C-ABI in include/coda_detr.h.
 #include <cuda_fp16.h>

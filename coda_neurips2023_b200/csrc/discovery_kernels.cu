@@ -1,4 +1,4 @@
-// Stage-2 novel-box discovery on the device (sm_100a): class-agnostic 2-D NMS of the projected boxes, rejection of
+// Stage-2 novel-box discovery on the device (sm_90a): class-agnostic 2-D NMS of the projected boxes, rejection of
 // boxes that overlap a ground-truth box in 3-D, objectness threshold, emitted as a fixed-capacity candidate list per
 // scene -- so that the step stays free of host synchronisation and CUDA-graph capturable.
 //

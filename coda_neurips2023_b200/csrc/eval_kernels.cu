@@ -1,4 +1,4 @@
-// Evaluation path on the device (sm_100a): what the reference's APCalculator does box by box on the host with numpy /
+// Evaluation path on the device (sm_90a): what the reference's APCalculator does box by box on the host with numpy /
 // scipy (utils/ap_calculator.py, utils/nms.py, utils/eval_det.py, utils/box_util.py) as four batched kernels.
 //
 //   points_in_boxes   -- "remove_empty_box": how many points of the scene lie inside each predicted box

@@ -1,4 +1,4 @@
-// PointNet++ set-abstraction ops for B200 (sm_100a) behind the C-ABI declared
+// PointNet++ set-abstraction ops for H100 (sm_90a) behind the C-ABI declared
 // in include/coda_pointnet2.h.  Written from the behaviour of the reference's
 // `pointnet2._ext` (third_party_pointnet2/pointnet2/_ext_src/src/*.cu), not
 // from its code: the reference runs one CTA per scene and one thread per ball
@@ -528,9 +528,9 @@ __global__ void three_interpolate_grad_kernel(int c, int n, int m, int c_per_blo
 }
 
 inline int pick_c_per_block(int c, long long work_items_per_channel, int b) {
-  // aim for >= ~4 waves of 148 SMs worth of 256-thread CTAs, at least 1 channel
+  // aim for >= ~4 waves of 132 SMs worth of 256-thread CTAs, at least 1 channel
   const long long ctas_per_channel_slice = (work_items_per_channel + 255) / 256 * b;
-  int slices = (int)((148LL * 8 + ctas_per_channel_slice - 1) / ctas_per_channel_slice);
+  int slices = (int)((132LL * 8 + ctas_per_channel_slice - 1) / ctas_per_channel_slice);
   if (slices < 1) slices = 1;
   if (slices > c) slices = c;
   return (c + slices - 1) / slices;

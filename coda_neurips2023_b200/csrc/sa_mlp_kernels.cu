@@ -1,4 +1,4 @@
-// Row-streaming kernels of the PointNet++ shared MLP for B200 (sm_100a): everything that sits between two
+// Row-streaming kernels of the PointNet++ shared MLP for H100 (sm_90a): everything that sits between two
 // tensor-core GEMMs of Conv1x1 -> BatchNorm -> ReLU blocks, one HBM pass each.  C-ABI in include/coda_sa_mlp.h.
 //
 // These kernels are HBM-bound by construction (a (1M, 256) fp32 activation is 1 GB): the design rule is to
@@ -16,7 +16,7 @@
 namespace {
 
 constexpr int THREADS = 256;
-constexpr int MAX_BLOCKS = 148 * 4;   // persistent-style grid: 4 resident blocks per SM
+constexpr int MAX_BLOCKS = 132 * 4;   // persistent-style grid: 4 resident blocks per SM of an H100 SXM
 
 __host__ __device__ inline bool channels_ok(int c) { return c >= 4 && c <= 1024 && c % 4 == 0 && THREADS % (c / 4) == 0; }
 
@@ -599,7 +599,7 @@ int coda_rows_colsum(long long rows, int c, const float *x, float *out, float *s
   cudaStream_t s = (cudaStream_t)stream;
   // short matrices: fewer blocks keep the second stage short
   unsigned grid = grid_for(rows, c);
-  if (grid > 148) grid = 148;
+  if (grid > 132) grid = 132;
   colsum_partial_kernel<<<grid, THREADS, 0, s>>>(rows, c, x, scratch);
   colsum_finalize_kernel<<<(c + 7) / 8, 256, 0, s>>>((int)grid, c, scratch, out);
   return coda::launch_status();
@@ -626,7 +626,7 @@ int coda_bn_relu_maxpool_rows(long long groups, int group, int c, const float *y
   if (groups < 0 || group < 1 || group > 256 || !channels_ok(c)) return CODA_EINVAL;
   if (groups == 0) return CODA_OK;
   if (!y || !mean || !invstd || !gamma || !beta || !pooled || !argmax) return CODA_EINVAL;
-  const unsigned grid = (unsigned)(groups < 148 * 8 ? groups : 148 * 8);
+  const unsigned grid = (unsigned)(groups < 132 * 8 ? groups : 132 * 8);
   bn_relu_maxpool_kernel<<<grid, THREADS, 0, (cudaStream_t)stream>>>(groups, group, c, y, mean, invstd, gamma, beta,
                                                                     pooled, argmax);
   return coda::launch_status();

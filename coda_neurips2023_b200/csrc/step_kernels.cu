@@ -1,4 +1,4 @@
-// Step-glue kernels for B200 (sm_100a): residual + dropout, BatchNorm(+ReLU+dropout) on channels-last rows
+// Step-glue kernels for H100 (sm_90a): residual + dropout, BatchNorm(+ReLU+dropout) on channels-last rows
 // with an fp32 result (the GenericMLP blocks), global-norm clip + AdamW on the flat parameter buffer.
 // All of them are pure streaming kernels over L2-resident or HBM-resident fp32 tensors: float4 per thread,
 // grid sized in multiples of the SM count, per-channel parameters in registers.  C-ABI in include/coda_step.h.
@@ -12,7 +12,7 @@
 namespace {
 
 constexpr int THREADS = 256;
-constexpr int NUM_SMS = 148;
+constexpr int NUM_SMS = 132;   // H100 SXM
 
 // ------------------------------------------------------------------ counter-based dropout mask
 // One 32-bit draw per element: lowbias32-style avalanche of (seed + index * odd).  Fwd and bwd call this with

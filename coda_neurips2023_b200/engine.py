@@ -1,7 +1,7 @@
 """One data-parallel training step: the body of the reference's training loop
 (engine.py:120-165 `train_one_epoch`: H2D of the batch, forward, criterion,
 backward with the gradient all-reduce, clip_grad_norm_, AdamW) as a reusable
-object, laid out for B200:
+object, laid out for the H100:
 
   * all trainable parameters live in ONE flat fp32 buffer and their gradients in another, ordered by
     the moment their gradient becomes final during the backward (measured once, on a probe pass), so

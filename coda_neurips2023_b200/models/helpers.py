@@ -2,7 +2,7 @@
 
 `NORM_DICT["ln"]` is the warp-per-row LayerNorm kernel (same parameters as nn.LayerNorm);
 GenericMLP keeps the reference's nn.Module tree (parameter paths `layers.{i}`) but executes on
-channels-last rows: tcgen05 GEMMs + one fused BatchNorm/ReLU/Dropout pass per block.
+channels-last rows: wgmma GEMMs + one fused BatchNorm/ReLU/Dropout pass per block.
 """
 from __future__ import annotations
 
@@ -89,7 +89,7 @@ class GenericMLP(nn.Module):
 
     def forward_rows(self, h):
         """The stack on channels-last rows (N, C_in) -> (N, C_out).  The 1x1 convolutions are GEMMs over the
-        channel dim (ops.linear, tcgen05); a [BatchNorm1d, ReLU, Dropout] run after a dense layer is ONE fused
+        channel dim (ops.linear, wgmma); a [BatchNorm1d, ReLU, Dropout] run after a dense layer is ONE fused
         pass over the rows (ops.bn_act_rows: batch statistics, normalise + ReLU + counter-based dropout); a ReLU
         directly after a dense layer runs in the GEMM epilogue."""
         mods = list(self.layers)

@@ -1,4 +1,4 @@
-"""CoDA's 3DETR detector with the CLIP alignment head, B200-native.
+"""CoDA's 3DETR detector with the CLIP alignment head, H100-native.
 
 Mirror of the registered model classes of reference models/model_3detr.py:
 `Model3DETRPredictedBoxDistillationHead` (:130-1833, CoDA proper),
@@ -11,7 +11,7 @@ work unchanged.
 
 What is different is how the step executes:
   * FPS / ball-query / grouping: cluster + ballot kernels (pointnet2/),
-  * attention: fused tcgen05 kernel, LayerNorm / Fourier encoding: warp kernels,
+  * attention: fused wgmma kernel, LayerNorm / Fourier encoding: warp kernels,
   * the CLIP crop pipeline (reference :984-1103: a Python double loop with four
     host syncs per box and one CLIP call per scene) is one batched projection in
     fp64 tensor ops, ONE crop+pad+bicubic-resize+normalise kernel for all B x 32

@@ -3,7 +3,7 @@ models/transformer.py: TransformerEncoder, TransformerEncoderLayer,
 MaskedTransformerEncoder, TransformerDecoder, TransformerDecoderLayer).
 
 Differences from the reference are implementation-only: attention runs in the
-fused tcgen05 kernel (no (B*H, L, L) probability tensor is written, no head
+fused wgmma kernel (no (B*H, L, L) probability tensor is written, no head
 averaging), LayerNorm is the warp-per-row kernel, and the K/V input projections
 of one packed weight are issued as single GEMMs.  Parameter names and shapes
 match `nn.MultiheadAttention` / the reference layers so checkpoints interchange.

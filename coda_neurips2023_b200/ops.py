@@ -1,6 +1,6 @@
 """torch-facing wrappers (autograd where needed) around the C-ABI kernels of
 include/coda_detr.h and include/coda_attention.h.  Every function here launches
-hand-written sm_100a code on the current stream; none has a CPU or PyTorch
+hand-written sm_90a code on the current stream; none has a CPU or PyTorch
 fallback -- a CPU tensor raises.
 """
 from __future__ import annotations
@@ -769,7 +769,7 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, nhead: int, dro
     q; the forward kernel never materialises the probabilities in HBM.
     """
     _need_cuda(q, "attention")
-    from . import attention_sm100  # tcgen05 kernels (include/coda_attention.h)
+    from . import attention_sm100  # wgmma kernels (include/coda_attention.h)
 
     return attention_sm100.attention(q, k, v, nhead, dropout_p, training, causal, mask)
 
@@ -840,7 +840,7 @@ def crop_resize_normalize(images: torch.Tensor, scene: torch.Tensor, boxes: torc
     return out
 
 
-# --------------------------------------------------------------------------- tcgen05 GEMM
+# --------------------------------------------------------------------------- wgmma GEMM
 # bf16 planes per fp32 operand.  3 -> six cross products, all 24 mantissa bits: fp32-class accuracy, which the
 # 1e-4 parity bar needs through 13 layers (2 planes / 3 products measured 1.4e-4 on the class logits).
 DEFAULT_NSPLIT = 3
@@ -912,7 +912,7 @@ def gemm_a32(a: torch.Tensor, b_planes: torch.Tensor, n: int, *, mode: int = A32
              alpha=None, beta=None, a2=None, argmax=None, group: int = 0, b_mn: bool = False, bias=None,
              relu: bool = False, out: torch.Tensor | None = None, want_stats: bool = False, nsplit: int | None = None):
     """C (m, n) = T(a) @ B^T with the fp32 activation `a` (m, k) read IN PLACE: the split into bf16 operand planes
-    happens inside the kernel (csrc/gemm_a32_sm100.cu), `T` is the prologue selected by `mode`
+    happens inside the kernel (csrc/gemm_a32_sm90.cu), `T` is the prologue selected by `mode`
     (include/coda_gemm.h).  b_planes: packed weight planes (nsplit, 1, rows, ld) -- K-major (rows = n) or, with
     b_mn, the forward planes of a weight (rows = k) reused for the input gradient.  Returns C, or (C, partials) with
     want_stats: per-CTA column sum / sum-of-squares partials of C for coda_bn_stats_finalize."""
@@ -951,7 +951,7 @@ def gemm_tn32(a: torch.Tensor, b: torch.Tensor, *, a_mode: int = A32_PLAIN, a_sc
               a_beta=None, a2=None, argmax=None, group: int = 0, b_mode: int = A32_PLAIN, b_scale=None,
               b_shift=None, out: torch.Tensor | None = None, colsum_out: torch.Tensor | None = None) -> torch.Tensor:
     """C (m, n) = sum_r TA(a)[r, :]^T TB(b)[r, :] from the fp32 activations a (R, m), b (R, n) read in place
-    (csrc/gemm_tn32_sm100.cu): the weight-gradient GEMM with the BatchNorm-backward / BatchNorm-forward
+    (csrc/gemm_tn32_sm90.cu): the weight-gradient GEMM with the BatchNorm-backward / BatchNorm-forward
     prologues applied inside the kernel.  Two bf16 planes per operand.  colsum_out (m,): receives sum_r TA(a)[r, :]
     (the bias gradient) from the same pass."""
     _need_cuda(a, "gemm_tn32")
@@ -995,7 +995,7 @@ BACKWARD_NSPLIT = 2
 USE_TN_WGRAD = True  # weight gradients from the row-packed operands (MN-major MMA); False: transposed packs
 
 
-# --------------------------------------------------------------------------- Linear on the tcgen05 GEMM
+# --------------------------------------------------------------------------- Linear on the wgmma GEMM
 _WEIGHT_EPOCH = 0
 _WEIGHT_CACHE: dict = {}
 # Weight planes depend on nothing but the parameters: a step can pack ALL of them up front on a side stream, under
@@ -1087,7 +1087,7 @@ def colsum(x: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
         return torch.sum(x, dim=0, out=out)
     if out is None:
         out = torch.empty(c, dtype=torch.float32, device=x.device)
-    scratch = torch.empty(148 * 4 * 2 * c, dtype=torch.float32, device=x.device)
+    scratch = torch.empty(132 * 4 * 2 * c, dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):
         st = lib().coda_rows_colsum(_ll(rows), _i(c), ptr(x), ptr(out), ptr(scratch), stream_of(x))
     check(st, "rows_colsum")
@@ -1095,7 +1095,7 @@ def colsum(x: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
 
 
 class _Linear(torch.autograd.Function):
-    """y = x W^T + b on the tcgen05 GEMM.  The activation is read IN PLACE as fp32 (gemm_a32: the bf16 split happens
+    """y = x W^T + b on the wgmma GEMM.  The activation is read IN PLACE as fp32 (gemm_a32: the bf16 split happens
     in the kernel's prologue); only the weight is packed (once per step, cached).  Backward: dX = dY W reuses the
     FORWARD weight planes as an MN-major operand (no transposed copy), dW = dY^T X runs on row-packed planes."""
 
@@ -1213,7 +1213,7 @@ def _bias_fp32(bias):
 
 def linear(x: torch.Tensor, weight: torch.Tensor, bias=None, relu: bool = False, nsplit: int | None = None,
            quick_gelu: bool = False, residual: torch.Tensor | None = None):
-    """y = x @ weight^T + bias over the last dim of x, on the tcgen05 GEMM (fp32 in / out, bf16
+    """y = x @ weight^T + bias over the last dim of x, on the wgmma GEMM (fp32 in / out, bf16
     split-operand accumulation); fp16 x / weight take the fp16 tensor-core path (inference only)."""
     _need_cuda(x, "linear")
     lead = x.shape[:-1]
@@ -1243,7 +1243,7 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias=None, relu: bool = False,
 
 
 class Linear(torch.nn.Linear):
-    """nn.Linear (same parameters / state-dict keys) running on the tcgen05 GEMM."""
+    """nn.Linear (same parameters / state-dict keys) running on the wgmma GEMM."""
 
     def forward(self, x):
         return linear(x, self.weight, self.bias)

@@ -83,7 +83,7 @@ class PointnetSAModuleVotes(nn.Module):
     Contract of reference pointnet2_modules.py:161-268:
         forward(xyz (B, N, 3), features (B, C, N) | None, inds (B, npoint) | None)
             -> new_xyz (B, npoint, 3), new_features (B, mlp[-1], npoint), inds (B, npoint) [, unique_cnt]
-    Hot path on B200: cluster FPS kernel -> gather -> fused ball-query/group/
+    Hot path on the H100: cluster FPS kernel -> gather -> fused ball-query/group/
     normalise kernel -> shared MLP -> max over the ball.
     """
 

@@ -107,7 +107,7 @@ def _batch_norm_rows(bn: nn.modules.batchnorm._BatchNorm, h: torch.Tensor) -> to
 class SharedMLP(nn.Sequential):
     """Stack of 1x1 Conv2d blocks: `layer0`, `layer1`, ... (reference
     pytorch_utils.py:8-33).  Executed channels-last: the (B, C, npoint, nsample) map is
-    (B*npoint*nsample, C) rows, each block one tcgen05 GEMM + BatchNorm over rows + ReLU."""
+    (B*npoint*nsample, C) rows, each block one wgmma GEMM + BatchNorm over rows + ReLU."""
 
     def forward(self, x):
         from .. import ops

@@ -5,7 +5,7 @@ ReLU blocks) followed by the `F.max_pool2d(kernel_size=[1, nsample])` of `Pointn
 (pointnet2_modules.py:247-254), on channels-last rows (B * npoint * nsample, C):
 
     layer 0      rows_linear_small_k (C_in = 3: exact fp32 FMAs)            -> y0
-    layer l > 0  tcgen05 split-bf16 GEMM on the planes written by layer l-1 -> y_l
+    layer l > 0  wgmma split-bf16 GEMM on the planes written by layer l-1 -> y_l
     between      BatchNorm statistics (one read of y_l), then normalise + ReLU + split into bf16 operand
                  planes in one pass (the fp32 activation is never written); the last layer instead folds
                  the max over the `nsample` rows of each seed in and returns (B * npoint, C) + arg-max

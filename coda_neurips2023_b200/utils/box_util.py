@@ -71,7 +71,7 @@ def generalized_box3d_iou(corners1, corners2, nums_k2, rotated_boxes: bool = Tru
     rectangles only for gt index < 4 (utils/box_intersection.pyx:181); the default
     computes every pair like the reference's TorchScript path."""
     if needs_grad or return_inter_vols_only:
-        raise NotImplementedError("differentiable GIoU (loss_giou_weight > 0) is not on the B200 path; "
+        raise NotImplementedError("differentiable GIoU (loss_giou_weight > 0) is not on the device path; "
                                   "every shipped CoDA script sets loss_giou_weight 0")
     rot = rotated_boxes if isinstance(rotated_boxes, torch.Tensor) else bool(rotated_boxes)
     return ops.giou3d(corners1.detach(), corners2.detach(), nums_k2, rot, rot_k2_limit)

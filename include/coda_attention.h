@@ -1,5 +1,5 @@
 /*
- * coda_attention.h -- C-ABI of the fused tcgen05 multi-head attention (forward and backward).
+ * coda_attention.h -- C-ABI of the fused wgmma multi-head attention (forward and backward).
  *
  * Replaces the attention core of torch.nn.MultiheadAttention as the reference calls it
  * in TransformerEncoderLayer / TransformerDecoderLayer (models/transformer.py:461-479,
@@ -61,7 +61,7 @@ int coda_attention_fwd_packed_ex(int b, int h, int lq, int lk, int hd, int nspli
 /*
  * fp16 self-attention with at most 64 tokens and head dim 64 (the CLIP ViT image tower, CLIP/clip/model.py:295-316 --
  * nn.MultiheadAttention on fp16 activations): q, k, v (l, b, h*64) IEEE half with row strides ld_* (slices of the fused
- * in-projection), out (l, b, h*64) half.  Operands stay half: one plane, one tcgen05.mma per product.
+ * in-projection), out (l, b, h*64) half.  Operands stay half: one plane, one wgmma per product.
  * workspace: 3 * b*h*l*64 halves + 256 bytes.
  */
 int coda_attention_fwd_half(int b, int h, int l, int hd, const void *q, const void *k, const void *v, long long ld_q,
@@ -87,7 +87,7 @@ int coda_attention_fwd_packed_masked(int b, int h, int lq, int lk, int hd, int n
                                      float dropout_p, unsigned int seed, const unsigned int *seed_dev, void *stream);
 
 /*
- * Backward of coda_attention_fwd (hd 64 or 128): two fused tcgen05 kernels (dQ row-wise; dK, dV
+ * Backward of coda_attention_fwd (hd 64 or 128): two fused wgmma kernels (dQ row-wise; dK, dV
  * column-wise) that recompute the probabilities from `lse`, regenerate the dropout mask from the same
  * counter stream, and never write an (Lq x Lk) tensor.
  *   q, k, v, out, dout as in the forward ((l, b, h*hd) fp32); lse (b*h, lq) from the forward;

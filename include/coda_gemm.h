@@ -1,5 +1,5 @@
 /*
- * coda_gemm.h -- C-ABI of the tcgen05 / TMA GEMM used for every dense layer on
+ * coda_gemm.h -- C-ABI of the wgmma / TMA GEMM used for every dense layer on
  * the path (Linear / 1x1-Conv of the 3DETR encoder, decoder and heads, the SA
  * shared MLP, and the CLIP ViT blocks).  In the reference these are
  * nn.Linear / nn.Conv1d / nn.Conv2d(1x1) calls into cuBLAS / cuDNN
@@ -11,7 +11,7 @@
  * of 64.  fp32 tensors are first split into nsplit bf16 planes by
  * coda_pack_split_bf16 (x = p0 + p1 (+ p2), each the bf16 rounding of what the
  * previous planes left over); the GEMM accumulates the 1 / 3 / 6 significant
- * cross products in fp32 in tensor memory.  nsplit = 2 carries ~16 mantissa
+ * cross products in fp32 registers.  nsplit = 2 carries ~16 mantissa
  * bits per operand, nsplit = 3 the full 24.
  */
 #ifndef CODA_GEMM_H
@@ -74,13 +74,13 @@ int coda_gemm_tn(int nsplit, int mc, int m, int n, const void *a, long long a_pl
                  const void *b, long long b_plane_stride, int ldb, float *c, long long ldc, void *stream);
 
 /*
- * GEMM with an FP32 A operand and an in-kernel prologue (csrc/gemm_a32_sm100.cu):
+ * GEMM with an FP32 A operand and an in-kernel prologue (csrc/gemm_a32_sm90.cu):
  *
  *     C (m, n) fp32 = T(A) (m, k) @ B^T  (+ bias) (ReLU)
  *
  * A is read as fp32 rows (row stride lda, multiple of 4 elements, 16-byte aligned base) by TMA, transformed
- * element-wise by T, split into `nsplit` (2 or 3) bf16 planes and handed to the tensor cores through tensor
- * memory -- no packed copy of A exists in HBM.  T (`a_mode`), with per-k vectors padded to a multiple of 64:
+ * element-wise by T, split into `nsplit` (2 or 3) bf16 planes and handed to the tensor cores as register
+ * operands -- no packed copy of A exists in HBM.  T (`a_mode`), with per-k vectors padded to a multiple of 64:
  *   CODA_A32_PLAIN          T = a                                   (every nn.Linear / 1x1 conv on the path)
  *   CODA_A32_AFFINE_RELU    T = relu(a * scale[k] + shift[k])       (BatchNorm(batch stats) + ReLU of the previous
  *                                                                    layer: pytorch_utils.py:8-33 SharedMLP blocks)
@@ -110,7 +110,7 @@ int coda_gemm_a32(int nsplit, int m, int n, int k, const float *a, long long lda
                   void *stream);
 
 /*
- * Weight-gradient form on fp32 rows with in-kernel prologues (csrc/gemm_tn32_sm100.cu):
+ * Weight-gradient form on fp32 rows with in-kernel prologues (csrc/gemm_tn32_sm90.cu):
  *
  *     C (m, n) fp32 = sum_r TA(A)[r][:m]^T TB(B)[r][:n],   A (rows, m) with row stride lda, B (rows, n) with ldb
  *

@@ -1,5 +1,5 @@
 /*
- * coda_pointnet2.h -- C-ABI of the B200-native PointNet++ set-abstraction ops.
+ * coda_pointnet2.h -- C-ABI of the H100-native PointNet++ set-abstraction ops.
  *
  * Drop-in boundary for the reference's pybind module `pointnet2._ext`
  * (third_party_pointnet2/pointnet2/_ext_src/src/bindings.cpp:9-22).  Every

@@ -8,7 +8,7 @@
  *   third_party_pointnet2/pointnet2/pointnet2_modules.py:248-254 (PointnetSAModuleVotes: F.max_pool2d over nsample)
  * which the reference runs as cuDNN convolution + ATen batch-norm / ReLU / pooling kernels, one full
  * pass over the (B * npoint * nsample, C) activation each.  Here the activation is kept channels-last
- * ("rows" = B * npoint * nsample, C channels), the convolutions are the split-bf16 tcgen05 GEMMs of
+ * ("rows" = B * npoint * nsample, C channels), the convolutions are the split-bf16 wgmma GEMMs of
  * coda_gemm.h, and everything between two GEMMs is ONE pass: normalise + ReLU + split into the bf16
  * operand planes the next GEMM reads (no fp32 intermediate is written), the last block folds the max
  * over neighbours in as well, and the backward mirrors it (mask + BatchNorm backward + operand planes

@@ -5,18 +5,19 @@ TEST INFRASTRUCTURE ONLY (see oracle/pointnet2_oracle.c header).
 Sources are compiled where they lie under
 /root/reference/third_party_pointnet2/pointnet2/_ext_src (never copied); the
 only outputs are ``oracle/_ref/pointnet2/_ext.so`` and an empty
-``oracle/_ref/pointnet2/__init__.py`` (``oracle/_ref/`` is git-ignored but NOT
-gpurun-ignored, so the binary travels to the B200 box where the GPU tests load
-it as ``pointnet2._ext`` and compare our kernels against it).
+``oracle/_ref/pointnet2/__init__.py`` (``oracle/_ref/`` is git-ignored; where the
+reference sources are absent, a prebuilt ``oracle/_ref`` is kept, and the GPU tests
+load it as ``pointnet2._ext`` to compare our kernels against it).
 
 This is a short recipe of direct nvcc / g++ calls -- the reference's own
 setup.py is not run.  The reference passes only ``-O2`` (setup.py:26-29) and gets
-its arch from torch; we pin ``compute_100/sm_100`` (plain, not 'a': the
+its arch from torch; we pin ``compute_90/sm_90`` (plain, not 'a': the
 reference has no arch-specific code).
 """
 from __future__ import annotations
 
 import concurrent.futures as cf
+import os
 import subprocess
 import sys
 from pathlib import Path
@@ -27,7 +28,7 @@ OBJ = OUT.parent / "obj"
 
 
 def main() -> int:
-    if not REF_SRC.exists():
+    if not os.path.isdir(REF_SRC):
         print("reference sources not present; keeping any prebuilt oracle/_ref", file=sys.stderr)
         return 0
     so = OUT / "_ext.so"
@@ -48,7 +49,7 @@ def main() -> int:
     def cc(src: Path) -> Path:
         obj = OBJ / (src.name + ".o")
         if src.suffix == ".cu":
-            cmd = ["nvcc", "-gencode", "arch=compute_100,code=sm_100", "-Xcompiler", "-fPIC",
+            cmd = ["nvcc", "-gencode", "arch=compute_90,code=sm_90", "-Xcompiler", "-fPIC",
                    "--expt-relaxed-constexpr", *common, *inc, "-c", str(src), "-o", str(obj)]
         else:
             cmd = ["g++", "-fPIC", *common, *inc, "-c", str(src), "-o", str(obj)]

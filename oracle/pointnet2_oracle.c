@@ -9,7 +9,7 @@
  * Parity pinning: the reference ships NO golden vectors for these ops
  * (SURVEY.md section 4); this restatement is pinned instead against the
  * reference's own CUDA extension compiled unmodified from /root/reference
- * (oracle/build_ref_ext.py -> oracle/_ref/) and run on the B200 box
+ * (oracle/build_ref_ext.py -> oracle/_ref/) and run on the GPU
  * (tests/test_pointnet2_gpu.py::test_*_vs_reference_ext), and the outputs of
  * that run are committed as fixtures under tests/golden/.
  *
@@ -42,7 +42,7 @@ static float sqdist_pt_minus_ref(float x2, float y2, float z2, float x1,
                                  float y1, float z1) {
   /* src/sampling_gpu.cu:106-107: (x2-x1)*(x2-x1)+(y2-y1)*(y2-y1)+(z2-z1)*(z2-z1).
    * nvcc (--fmad=true) contracts a*a + b*b + c*c as FMUL(b,b); FFMA(a,a,.);
-   * FFMA(c,c,.) -- read off the SASS of the reference build for sm_100
+   * FFMA(c,c,.) -- read off the SASS of the reference build
    * (cuobjdump -sass oracle/_ref/obj/sampling_gpu.cu.o): the SECOND product is
    * the plain multiply. */
   const float dx = x2 - x1, dy = y2 - y1, dz = z2 - z1;

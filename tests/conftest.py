@@ -15,7 +15,7 @@ os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the GPU with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -5,7 +5,7 @@ patch 32, 50 tokens), name-keyed random weights rounded to fp16 exactly as `conv
 
   * in fp32 arithmetic on those fp16 weights  -> `cls32` / `tok32`: the infinitely-precise answer,
   * in fp16 arithmetic (what the reference executes on a GPU)  -> `cls16`: how far the reference's own
-    fp16 run sits from that answer; the parity test holds our fp16 tcgen05 tower to the same distance.
+    fp16 run sits from that answer; the parity test holds our fp16 wgmma tower to the same distance.
 
 Weights are not stored (tests/param_fill.py regenerates them by name), the 32 input crops are (seeded,
 fp16-rounded CLIP-normalised pixels).

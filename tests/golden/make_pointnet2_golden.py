@@ -1,8 +1,7 @@
 """Generates tests/golden/pointnet2_ref_*.npz from the REFERENCE's own CUDA extension.
 
-Run on the B200 box (the reference extension has no CPU path):
-    python tests/golden/make_pointnet2_golden.py gpurun_out/golden
-then copy the files into tests/golden/.  Inputs are regenerated from the seed by
+Run on a GPU (the reference extension has no CPU path), with the extension built by oracle/build_ref_ext.py:
+    python tests/golden/make_pointnet2_golden.py [OUT_DIR]        (default: tests/golden/)  Inputs are regenerated from the seed by
 coda_neurips2023_b200.synthetic.point_clouds, so only outputs are stored.
 """
 import importlib
@@ -45,4 +44,4 @@ def main(out_dir: str):
 
 
 if __name__ == "__main__":
-    main(sys.argv[1] if len(sys.argv) > 1 else "gpurun_out/golden")
+    main(sys.argv[1] if len(sys.argv) > 1 else str(Path(__file__).resolve().parent))

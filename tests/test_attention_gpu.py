@@ -1,4 +1,4 @@
-"""Fused tcgen05 attention forward against a float64 softmax(QK^T)V of the same inputs."""
+"""Fused wgmma attention forward against a float64 softmax(QK^T)V of the same inputs."""
 import pytest
 import torch
 

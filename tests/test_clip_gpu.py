@@ -1,4 +1,4 @@
-"""The benchmarked CLIP image tower -- ViT-B/32, 12 layers, fp16 weights, fp16 tcgen05 GEMMs + the single-tile
+"""The benchmarked CLIP image tower -- ViT-B/32, 12 layers, fp16 weights, fp16 wgmma GEMMs + the single-tile
 fused attention + the fp16 LayerNorm kernel -- against the REFERENCE's own VisionTransformer
 (CLIP/clip/model.py:593-659) on the same name-keyed fp16-rounded weights and the same 32 crops
 (tests/golden/clip_vit_b32.npz, made by tests/golden/make_clip_vit_golden.py from /root/reference).

@@ -1,6 +1,7 @@
 """The package's CLIP tokenizer against token rows produced by the reference's own tokenizer
 (tests/golden/clip_tokens.npz, written by tests/golden/make_clip_tokens_golden.py).  The BPE vocabulary is a
-data file of a CoDA checkout, not of this package: the test runs where one is reachable."""
+data file of a CoDA checkout, not of this package; tests/golden/clip_bpe_merges_48894.txt.gz holds the part of
+CLIP's bpe_simple_vocab_16e6.txt.gz the tokenizer reads (the header line and the first 49152 - 256 - 2 merges)."""
 import os
 from pathlib import Path
 
@@ -11,8 +12,7 @@ import torch
 from coda_neurips2023_b200.clip import tokenizer
 
 GOLDEN = Path(__file__).parent / "golden" / "clip_tokens.npz"
-CANDIDATES = [os.environ.get("CODA_CLIP_BPE", ""), "/root/reference/CLIP/clip/bpe_simple_vocab_16e6.txt.gz",
-              "CLIP/clip/bpe_simple_vocab_16e6.txt.gz"]
+CANDIDATES = [os.environ.get("CODA_CLIP_BPE", ""), str(Path(__file__).parent / "golden" / "clip_bpe_merges_48894.txt.gz")]
 
 
 def _vocab():

@@ -1,7 +1,6 @@
 """CPU side of the device data layer: the numpy restatement (oracle/data_ref.py) is pinned to the REFERENCE's own
 RandomCuboid (utils/random_cuboid.py) fed the same random draws, and its sampler is checked for the properties
 np.random.choice guarantees (distinct rows, inside the crop, uniform)."""
-import sys
 from pathlib import Path
 
 import numpy as np
@@ -10,10 +9,11 @@ import pytest
 import data_ref
 from coda_neurips2023_b200 import synthetic
 
-REF = Path("/root/reference")
+GOLDEN = Path(__file__).resolve().parent / "golden" / "random_cuboid_ref.npz"
+CASES = [(0, 1500), (1, 3000), (2, 5900), (3, 100)]
 
 
-def _scene(seed, n=6000, g=7):
+def scene(seed, n=6000, g=7):
     rng = np.random.default_rng(seed)
     pts = synthetic.point_clouds(1, n, seed=seed)[0].astype(np.float32)
     boxes = np.zeros((g, 8), np.float32)
@@ -24,40 +24,24 @@ def _scene(seed, n=6000, g=7):
     return pts, boxes
 
 
-@pytest.mark.skipif(not REF.exists(), reason="needs the reference checkout (this container only)")
-@pytest.mark.parametrize("seed,min_points", [(0, 1500), (1, 3000), (2, 5900), (3, 100)])
-def test_random_cuboid_restatement_equals_reference_with_replayed_draws(seed, min_points):
-    """utils/random_cuboid.py draws np.random.rand(3) per attempt and np.random.choice(n) when the aspect test
-    passes; replaying a table through both gives the same crop, the same kept points and the same kept boxes."""
-    sys.path.insert(0, str(Path(__file__).resolve().parent / "golden"))
-    import _reference_harness as H
-
-    rc = H.load("utils.random_cuboid")
-    pts, boxes = _scene(seed)
+def replay_table(seed, ncand=100):
+    """the candidate crops both sides draw from: crop ranges and centre draws of `ncand` attempts"""
     rng = np.random.default_rng(100 + seed)
-    ncand = 100
     crop_range = 0.5 + rng.random((ncand, 3)) * 0.5
     center_u = rng.random(ncand).astype(np.float32)
+    return crop_range, center_u
 
-    class Replay:
-        k = -1
 
-        @classmethod
-        def rand(cls, n):
-            cls.k += 1
-            return (crop_range[cls.k] - 0.5) * 2.0           # exact: min_crop + r * (max_crop - min_crop) = crop_range
-
-        @classmethod
-        def choice(cls, n):
-            return data_ref.center_index(center_u[cls.k], n)
-
-    aug = rc.RandomCuboid(min_points=min_points, aspect=0.8, min_crop=0.5, max_crop=1.0)
-    saved = rc.np.random.rand, rc.np.random.choice
-    rc.np.random.rand, rc.np.random.choice = Replay.rand, Replay.choice
-    try:
-        ref_pts, ref_boxes, _ = aug(pts.copy(), boxes.copy())
-    finally:
-        rc.np.random.rand, rc.np.random.choice = saved
+@pytest.mark.parametrize("seed,min_points", CASES)
+def test_random_cuboid_restatement_equals_reference_with_replayed_draws(seed, min_points):
+    """utils/random_cuboid.py draws np.random.rand(3) per attempt and np.random.choice(n) when the aspect test
+    passes; replaying a table through both gives the same crop, the same kept points and the same kept boxes.  The
+    reference's side of the comparison is stored in tests/golden/random_cuboid_ref.npz
+    (tests/golden/make_random_cuboid_golden.py)."""
+    golden = np.load(GOLDEN)
+    ref_pts, ref_boxes = golden[f"pts_{seed}_{min_points}"], golden[f"boxes_{seed}_{min_points}"]
+    pts, boxes = scene(seed)
+    crop_range, center_u = replay_table(seed)
     chosen, crop, keep = data_ref.random_cuboid(pts, boxes, crop_range, center_u, min_points, aspect=0.8)
     inside = np.all(pts[:, :3].astype(np.float64) <= crop[3:], axis=1) & np.all(pts[:, :3].astype(np.float64) >= crop[:3], axis=1)
     assert np.array_equal(pts[inside], ref_pts)
@@ -69,7 +53,7 @@ def test_random_cuboid_restatement_equals_reference_with_replayed_draws(seed, mi
 
 
 def test_feistel_sampler_draws_distinct_rows_uniformly():
-    pts, _ = _scene(5, n=5000)
+    pts, _ = scene(5, n=5000)
     crop = np.array([-2.0, 0.8, -1.1, 2.5, 5.0, 1.2])
     inside = np.all(pts[:, :3] <= crop[3:], axis=1) & np.all(pts[:, :3] >= crop[:3], axis=1)
     m = int(inside.sum())
@@ -90,7 +74,7 @@ def test_feistel_sampler_draws_distinct_rows_uniformly():
 
 
 def test_scene_transform_is_the_reference_formula_in_float32():
-    pts, _ = _scene(7, n=2000)
+    pts, _ = scene(7, n=2000)
     ang = 0.3
     rot = np.array([[np.cos(ang), -np.sin(ang), 0], [np.sin(ang), np.cos(ang), 0], [0, 0, 1.0]])
     got = data_ref.scene_transform(pts, -1.0, rot, 1.1)

@@ -1,4 +1,4 @@
-"""The fp32-A tcgen05 GEMM with in-kernel prologues (include/coda_gemm.h, coda_gemm_a32) against fp64 references:
+"""The fp32-A wgmma GEMM with in-kernel prologues (include/coda_gemm.h, coda_gemm_a32) against fp64 references:
 plain, BatchNorm+ReLU prologue, the two BatchNorm-backward prologues, K-major and MN-major weights, ragged m / n / k,
 and the column-statistics epilogue."""
 import numpy as np
@@ -120,6 +120,12 @@ def test_tn32_plain_matches_fp64(rows, m, n):
     got = ops.gemm_tn32(a, b)
     exp = a.double().t() @ b.double()
     assert _rel(got, exp) < 6e-5
+    # split-K over the rows: partial tiles and column sums are added in split order, the same bits on every call
+    cs1, cs2 = torch.empty(m, device="cuda"), torch.empty(m, device="cuda")
+    got1 = ops.gemm_tn32(a, b, colsum_out=cs1)
+    assert torch.equal(got1, got)
+    assert torch.equal(ops.gemm_tn32(a, b, colsum_out=cs2), got1) and torch.equal(cs1, cs2)
+    torch.testing.assert_close(cs1.double(), a.double().sum(0), rtol=1e-5, atol=1e-3)
 
 
 def test_tn32_bn_backward_and_forward_prologues():

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (include/coda_gemm.h) against a float64 matmul of the same operands."""
+"""wgmma GEMM (include/coda_gemm.h) against a float64 matmul of the same operands."""
 import pytest
 import torch
 
@@ -84,6 +84,24 @@ def test_gemm_split_k_weight_gradient_shape():
     dw = ops.gemm_nt(dyt, xt, n, k)[0]
     ref = dy.double().t() @ x.double()
     assert ((dw.double() - ref).abs().max() / ref.abs().max()).item() < 1e-5
+    # the splits' partial tiles are added in a fixed order: the same bits on every call
+    assert torch.equal(ops.gemm_nt(dyt, xt, n, k)[0], dw)
+
+
+def test_gemm_split_k_after_a_larger_split_k_launch():
+    """The split-K scratch is shared: a larger launch first leaves non-zero partial tiles in it.  A shape whose
+    k-blocks do not divide evenly among the splits (9 output tiles over 16384 contraction columns) must still read
+    only the partials it wrote itself."""
+    torch.manual_seed(3)
+    x = torch.randn(200000, 64, device="cuda")
+    dy = torch.randn(200000, 128, device="cuda")
+    ops.gemm_nt(ops.pack_split(dy, 128, 200000, 1, 128, 3), ops.pack_split(x, 64, 200000, 1, 64, 3), 128, 64)
+    m, n, k = 384, 384, 16384
+    a = torch.randn(m, k, device="cuda")
+    b = torch.randn(n, k, device="cuda")
+    c = ops.gemm_nt(ops.pack_split(a, m, k, k, 1, 3), ops.pack_split(b, n, k, k, 1, 3), m, n)[0]
+    ref = a.double() @ b.double().t()
+    assert ((c.double() - ref).abs().max() / ref.abs().max()).item() < 1e-5
 
 
 def test_linear_autograd_matches_torch():

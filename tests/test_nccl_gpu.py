@@ -116,7 +116,7 @@ def _worker(rank, world, port, ret, sync_bn=False):
     os._exit(0)       # a live CUDA graph references the communicator: do not tear NCCL down
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_two_rank_step_equals_concatenated_batch(built_lib):
     import torch.multiprocessing as mp
 
@@ -176,7 +176,7 @@ def _single_gpu_train_bn_grads(perm):
     return grads, means
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_two_rank_sync_batchnorm_equals_concatenated_batch(built_lib):
     """TrainStep(sync_bn=True): BatchNorm in TRAINING mode with statistics all-reduced over the ranks (the
     reference's convert_sync_batchnorm, main.py:993).  Two ranks x 2 scenes must then give the gradient -- and the
@@ -214,5 +214,4 @@ def test_two_rank_sync_batchnorm_equals_concatenated_batch(built_lib):
     print(f"PARITY nccl_2rank_syncbn: worst deviation / (6 x reorder noise, floor 3e-3) = {worst_excess:.2f}, "
           f"running-mean deviation {stat:.2e}")
     assert stat < 1e-4
-    # measured on 2 x B200 (round-2 head): worst ratio 0.15, i.e. every parameter well inside its own reorder noise
     assert worst_excess < 1.0

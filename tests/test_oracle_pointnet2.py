@@ -1,6 +1,6 @@
 """CPU tests (no GPU): the C oracle against hand-checkable cases, against an
 independent numpy formulation of the same rules, and against the golden vectors
-produced by the reference's own CUDA extension on the B200 box
+produced by the reference's own CUDA extension on the GPU
 (tests/golden/pointnet2_ref_*.npz, written by tests/golden/make_pointnet2_golden.py)."""
 from pathlib import Path
 
@@ -185,7 +185,7 @@ def _golden_files():
 @pytest.mark.skipif(not _golden_files(), reason="reference-extension golden vectors not generated yet")
 @pytest.mark.parametrize("path", _golden_files(), ids=lambda p: p.stem)
 def test_oracle_matches_reference_extension_golden(path):
-    """Pins the oracle: outputs of the UNMODIFIED reference CUDA extension on B200."""
+    """Pins the oracle: outputs of the UNMODIFIED reference CUDA extension on the GPU."""
     z = np.load(path)
     xyz = synthetic.point_clouds(int(z["batch"]), int(z["n"]), seed=int(z["seed"]),
                                  dup_frac=float(z["dup_frac"]))

@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a kernels (through the C-ABI / `_ext` binding)
+"""GPU parity tests: the sm_90a kernels (through the C-ABI / `_ext` binding)
 against the CPU oracle, against the reference's own CUDA extension when its
 build travelled with the snapshot (oracle/_ref), and against the golden vectors.
 Bar: bit-exact for indices and for pure copies; 1e-5 for atomically accumulated

@@ -20,7 +20,8 @@ def test_dropout_add_mask_is_shared_by_forward_and_backward():
     from coda_neurips2023_b200 import attention_launch, ops
 
     torch.manual_seed(0)
-    x = torch.randn(2048, 8, 256, device="cuda", requires_grad=True)
+    x = torch.randn(2048, 8, 256, device="cuda")
+    x = x.masked_fill(x == 0, 1.0).requires_grad_()   # the mask is read off delta / x below: no exact zeros in x
     r = torch.randn_like(x, requires_grad=True)
     attention_launch.advance_seed(x.device)
     out = ops.dropout_add(x, r, 0.1, True)

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the fused attention kernels on the training step's shapes (B200).
+"""Micro-benchmark of the fused attention kernels on the training step's shapes (H100).
 
     python tools/bench_attention.py            # one JSON line per case
 """

@@ -1,4 +1,4 @@
-"""Throughput of the tcgen05 GEMM (packed operands resident) vs torch.matmul fp32 / bf16."""
+"""Throughput of the wgmma GEMM (packed operands resident) vs torch.matmul fp32 / bf16."""
 import json
 import sys
 from pathlib import Path

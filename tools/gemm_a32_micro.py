@@ -1,6 +1,5 @@
-"""Micro-benchmark of the fp32-A tcgen05 GEMMs (CUDA events, kernel alone, warm) on the step's shapes.
-Prints one JSON line per case: ms, useful TFLOP/s, algorithmic GB/s.  Also the subject of the ncu captures in
-profiles/ (`ncu --set full -k regex:gemm_a32 ...`)."""
+"""Micro-benchmark of the fp32-A wgmma GEMMs (CUDA events, kernel alone, warm) on the step's shapes.
+Prints one JSON line per case: ms, useful TFLOP/s, algorithmic GB/s."""
 import json
 import sys
 from pathlib import Path

@@ -5,8 +5,7 @@ neighbours) forward + backward at the BASELINE size (8 scenes x 2048 seeds x 64 
         --csv --log-file out.csv python tools/sa_mlp_traffic.py
     python tools/sa_mlp_traffic.py --summarise out.csv      -> total bytes / time per direction
 
-Works with any revision of the package on PYTHONPATH (the round-1 tree is measured the same way for the
-before / after comparison in profiles/)."""
+Works with any revision of the package on PYTHONPATH, so two revisions can be compared the same way."""
 import csv
 import sys
 from pathlib import Path
