@@ -17,8 +17,15 @@
 // S is recomputed in both kernels so that every accumulation stays inside one CTA: no atomics, deterministic.
 // Operands are split-bf16 planes like the forward; the backward uses 2 planes (3 cross products, ~16 mantissa
 // bits), enough for the 2e-3 gradient parity bar.  Only row-major packs of q, k, v, dO are needed (no transposed
-// copies).  Head dim 128 runs one warpgroup per CTA: its accumulators (dK and dV, or dQ, plus S and dP) need the
+// copies).  Head dim 128 runs one MMA warpgroup per CTA: its accumulators (dK and dV, or dQ, plus S and dP) need the
 // register file of a one-warpgroup CTA.
+//
+// Both kernels: NWG MMA warpgroups + one TMA producer warpgroup.  With two MMA warpgroups the producer hands its
+// registers to them (setmaxnreg: 24 / 240 per thread instead of 168 for all).  The dK/dV kernel holds no per-query
+// values in registers: log-sum-exp and D of the 64 queries of a tile arrive in shared memory with the tile (one bulk
+// copy of a padded (lse log2 e, D) array that the D kernel writes), and the dropout stream seed of a query is hashed
+// when its column is converted.  So its two accumulators, S and dP fit without spilling, and the wgmmas that read
+// them are not serialised.
 // Optional attention mask (bit-packed, 1 = key not visible to query; MaskedTransformerEncoder of the reference,
 // models/transformer.py:146-211): one 64-bit word per (row, 64-column tile).
 #include "../../include/coda_attention.h"
@@ -32,19 +39,26 @@ namespace {
 constexpr int NS = 2;           // planes per operand in the backward
 constexpr int NPROD = 3;
 
-// D[bh][q] = sum_d dO * O   (both (Lq, B, H*hd)); one warp per (q, b, h)
+// Per-query values of the backward, qv[bh][q] = (lse * log2 e, D = sum_d dO * O) with dO, O (Lq, B, H*hd); rows
+// Lq..Lqp-1 (padding to whole 64-query tiles) are zero, so a tile's 64 entries are one aligned 512-byte block.
+// One warp per (q, b, h).
 __global__ void __launch_bounds__(256)
-bwd_delta_kernel(int Lq, int B, int H, int hd, const float *__restrict__ dout, const float *__restrict__ out,
-                 float *__restrict__ delta) {
+bwd_delta_kernel(int Lq, int Lqp, int B, int H, int hd, const float *__restrict__ dout, const float *__restrict__ out,
+                 const float *__restrict__ lse, float2 *__restrict__ qv) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (warp >= Lq * B * H) return;
+  if (warp >= Lqp * B * H) return;
   const int h = warp % H, b = (warp / H) % B, q = warp / (H * B);
+  const size_t row = (size_t)(b * H + h) * Lqp + q;
+  if (q >= Lq) {
+    if (lane == 0) qv[row] = make_float2(0.f, 0.f);
+    return;
+  }
   const size_t off = ((size_t)q * B + b) * H * hd + (size_t)h * hd;
   float s = 0.f;
   for (int d = lane; d < hd; d += 32) s += __ldg(dout + off + d) * __ldg(out + off + d);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if (lane == 0) delta[(size_t)(b * H + h) * Lq + q] = s;
+  if (lane == 0) qv[row] = make_float2(__ldg(lse + (size_t)(b * H + h) * Lq + q) * LOG2E, s);
 }
 
 struct BwdMaps {
@@ -58,7 +72,8 @@ __device__ __forceinline__ float ex2_approx_b(float x) {
 }
 
 // Shared-memory plan of both kernels: RES = the CTA's resident rows (two operands x NS planes x NWG 64-row boxes per
-// 64 head-dim columns), then NST stages of the streamed 64-row tiles (two operands x NS planes).
+// 64 head-dim columns), then NST stages of the streamed 64-row tiles (two operands x NS planes), then (dK/dV kernel)
+// the per-query (lse log2 e, D) block of each stage.
 template <int HD, int NWG>
 struct BwdCfg {
   static constexpr int KB = HD / 64;
@@ -69,16 +84,23 @@ struct BwdCfg {
   static constexpr int STAGE = 2 * NS * TILE_PLANE;
   static constexpr int NST_FIT = (220 * 1024 - RES) / STAGE;
   static constexpr int NST = NST_FIT > 4 ? 4 : NST_FIT;
-  static constexpr int TOTAL = RES + NST * STAGE;
-  static constexpr int THREADS = NWG * 128 + 32;
+  static constexpr int QV = RES + NST * STAGE;        // NST x 64 float2
+  static constexpr int QV_STAGE = 64 * 8;
+  static constexpr int TOTAL = QV + NST * QV_STAGE;
+  static constexpr int THREADS = (NWG + 1) * 128;     // NWG MMA warpgroups, then the producer warpgroup
+  // per-thread registers after the producer hands its share over (NWG == 1: 255 already, nothing to move)
+  static constexpr int PRODUCER_REGS = 24, MMA_REGS = 240;
+  static_assert(NWG == 1 || PRODUCER_REGS * 128 + MMA_REGS * 128 * NWG <= 65536, "register file");
   static_assert(NST >= 1 && TOTAL + 1024 <= 227 * 1024, "smem budget");
 };
 
 // the two 64 x 64 score-side products X Y^T of one tile (X resident rows of the warpgroup, Y a streamed tile):
-// s = X0 Y0^T, t = X1 Y1^T over NS planes x KB head-dim blocks
+// s = X0 Y0^T, t = X1 Y1^T over NS planes x KB head-dim blocks.  Issued as one committed wgmma group; the caller
+// waits for it.
 template <int KB>
-__device__ __forceinline__ void scores2(float (&s)[32], float (&t)[32], const unsigned char *x0, const unsigned char *y0,
-                                        const unsigned char *x1, const unsigned char *y1, int res_plane, int tile_plane) {
+__device__ __forceinline__ void scores2_issue(float (&s)[32], float (&t)[32], const unsigned char *x0,
+                                              const unsigned char *y0, const unsigned char *x1, const unsigned char *y1,
+                                              int res_plane, int tile_plane) {
   acc_fence(s);
   acc_fence(t);
   wgmma_fence();
@@ -98,17 +120,14 @@ __device__ __forceinline__ void scores2(float (&s)[32], float (&t)[32], const un
       }
     }
   wgmma_commit();
-  wgmma_wait<0>();
-  acc_fence(s);
-  acc_fence(t);
 }
 
 // ====================================================================== dQ
 template <int HD, int NWG>
 __global__ void __launch_bounds__(BwdCfg<HD, NWG>::THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B, int H, float scale,
-                   const float *__restrict__ lse, const float *__restrict__ delta, float *__restrict__ dq,
-                   long long ld_dq, const unsigned long long *__restrict__ mask_q, float drop_p, uint32_t seed,
+                   const float2 *__restrict__ qv, float *__restrict__ dq, long long ld_dq,
+                   const unsigned long long *__restrict__ mask_q, float drop_p, uint32_t seed,
                    const uint32_t *__restrict__ seed_dev) {
   using C = BwdCfg<HD, NWG>;
   constexpr int KB = C::KB, NST = C::NST;
@@ -127,8 +146,10 @@ attn_bwd_dq_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B, 
   }
   __syncthreads();
 
-  if (warp == NWG * 4) {
-    // ===== TMA producer (warp-uniform control flow, one elected lane issues) =====
+  if (warp >= NWG * 4) {
+    // ===== TMA producer warpgroup: its first warp issues (warp-uniform control flow, one elected lane) =====
+    if constexpr (NWG > 1) setmaxnreg_dec<C::PRODUCER_REGS>();
+    if (warp != NWG * 4) return;
     if (elect_one_sync()) {
       mbar_arrive_expect_tx(&q_full, (uint32_t)C::RES);
 #pragma unroll
@@ -161,16 +182,19 @@ attn_bwd_dq_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B, 
     }
     return;
   }
+  if constexpr (NWG > 1) setmaxnreg_inc<C::MMA_REGS>();
 
   const int w = warp >> 2, wl = warp & 3, g = lane >> 2, t4 = lane & 3;
   const int qrow[2] = {q0 + 64 * w + wl * 16 + g, q0 + 64 * w + wl * 16 + g + 8};
+  const int Lqp = (Lq + 63) & ~63;
   float lse2[2], d_r[2];
   const unsigned long long *mrow[2];
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     const bool valid = qrow[i] < Lq;
-    lse2[i] = (valid ? __ldg(lse + (size_t)bh * Lq + qrow[i]) : 0.f) * LOG2E;
-    d_r[i] = valid ? __ldg(delta + (size_t)bh * Lq + qrow[i]) : 0.f;
+    const float2 v = valid ? __ldg(qv + (size_t)bh * Lqp + qrow[i]) : make_float2(0.f, 0.f);
+    lse2[i] = v.x;
+    d_r[i] = v.y;
     mrow[i] = mask_q ? mask_q + ((size_t)(bh / H) * Lq + (valid ? qrow[i] : 0)) * (size_t)ntiles : nullptr;
   }
   const bool dropout = drop_p > 0.f;
@@ -185,7 +209,10 @@ attn_bwd_dq_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B, 
     const unsigned char *ks = smem + C::RES + st * C::STAGE, *vs = ks + NS * C::TILE_PLANE;
     mbar_wait(&kv_full[st], (uint32_t)(j / NST) & 1u);
     float sacc[32], pacc[32];
-    scores2<KB>(sacc, pacc, qs, ks, dos, vs, C::RES_PLANE, C::TILE_PLANE);
+    scores2_issue<KB>(sacc, pacc, qs, ks, dos, vs, C::RES_PLANE, C::TILE_PLANE);
+    wgmma_wait<0>();
+    acc_fence(sacc);
+    acc_fence(pacc);
     const int kvalid = Lk - j * 64;
     uint32_t af[4][NS][4];
 #pragma unroll
@@ -241,8 +268,8 @@ attn_bwd_dq_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B, 
 template <int HD, int NWG>
 __global__ void __launch_bounds__(BwdCfg<HD, NWG>::THREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B, int H,
-                    const float *__restrict__ lse, const float *__restrict__ delta, float *__restrict__ dk,
-                    float *__restrict__ dv, long long ld_dk, long long ld_dv,
+                    const float2 *__restrict__ qv, float *__restrict__ dk, float *__restrict__ dv, long long ld_dk,
+                    long long ld_dv,
                     const unsigned long long *__restrict__ mask_k, float drop_p, uint32_t seed,
                     const uint32_t *__restrict__ seed_dev) {
   using C = BwdCfg<HD, NWG>;
@@ -254,7 +281,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B,
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int k0 = blockIdx.x * 64 * NWG, bh = blockIdx.y;
   const int ntiles = (Lq + 63) / 64;
-  // resident: K planes at 0, V planes at NS * RES_PLANE;  stage: Qs planes, then dO planes
+  // resident: K planes at 0, V planes at NS * RES_PLANE;  stage: Qs planes, then dO planes; QV: per-query values
   if (threadIdx.x == 0) {
     mbar_init(&kv_full, 1);
     for (int i = 0; i < NST; ++i) { mbar_init(&q_full[i], 1); mbar_init(&q_empty[i], NWG); }
@@ -262,7 +289,10 @@ attn_bwd_dkv_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B,
   }
   __syncthreads();
 
-  if (warp == NWG * 4) {
+  if (warp >= NWG * 4) {
+    // ===== TMA producer warpgroup: its first warp issues =====
+    if constexpr (NWG > 1) setmaxnreg_dec<C::PRODUCER_REGS>();
+    if (warp != NWG * 4) return;
     if (elect_one_sync()) {
       mbar_arrive_expect_tx(&kv_full, (uint32_t)C::RES);
 #pragma unroll
@@ -281,7 +311,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B,
       const int st = i % NST;
       mbar_wait(&q_empty[st], ((uint32_t)(i / NST) & 1u) ^ 1u);
       if (elect_one_sync()) {
-        mbar_arrive_expect_tx(&q_full[st], (uint32_t)C::STAGE);
+        mbar_arrive_expect_tx(&q_full[st], (uint32_t)(C::STAGE + C::QV_STAGE));
         unsigned char *sb = smem + C::RES + st * C::STAGE;
 #pragma unroll
         for (int p = 0; p < NS; ++p)
@@ -290,11 +320,13 @@ attn_bwd_dkv_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B,
             tma_load_3d(sb + (p * KB + kb) * C::BOX, &maps.q[p], &q_full[st], kb * 64, i * 64, bh);
             tma_load_3d(sb + NS * C::TILE_PLANE + (p * KB + kb) * C::BOX, &maps.dO[p], &q_full[st], kb * 64, i * 64, bh);
           }
+        bulk_load_1d(smem + C::QV + st * C::QV_STAGE, qv + ((size_t)bh * ntiles + i) * 64, C::QV_STAGE, &q_full[st]);
       }
       __syncwarp();
     }
     return;
   }
+  if constexpr (NWG > 1) setmaxnreg_inc<C::MMA_REGS>();
 
   const int w = warp >> 2, wl = warp & 3, g = lane >> 2, t4 = lane & 3;
   const int krow[2] = {k0 + 64 * w + wl * 16 + g, k0 + 64 * w + wl * 16 + g + 8};
@@ -318,41 +350,41 @@ attn_bwd_dkv_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B,
   for (int it = 0; it < ntiles; ++it) {
     const int st = it % NST;
     const unsigned char *qs = smem + C::RES + st * C::STAGE, *dos = qs + NS * C::TILE_PLANE;
-    // the per-query values of this thread's 16 columns: log-sum-exp (log2 units), D, dropout stream seeds
-    float lse16[16], dl16[16];
-    uint32_t sd16[16];
+    // (lse log2 e, D) of the tile's 64 queries
+    const float2 *qvs = reinterpret_cast<const float2 *>(smem + C::QV + st * C::QV_STAGE);
+    unsigned long long mb[2];
 #pragma unroll
-    for (int c = 0; c < 8; ++c)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int qi = it * 64 + c * 8 + 2 * t4 + e;
-        const bool ok = qi < Lq;
-        lse16[c * 2 + e] = ok ? __ldg(lse + (size_t)bh * Lq + qi) * LOG2E : 0.f;
-        dl16[c * 2 + e] = ok ? __ldg(delta + (size_t)bh * Lq + qi) : 0.f;
-        sd16[c * 2 + e] = dropout ? drop_tile_seed(seed, (uint32_t)bh, (uint32_t)qi, ktile) : 0u;
-      }
+    for (int i = 0; i < 2; ++i) mb[i] = mrow[i] ? __ldg(mrow[i] + it) : 0ull;
     mbar_wait(&q_full[st], (uint32_t)(it / NST) & 1u);
     float sacc[32], pacc[32];
-    scores2<KB>(sacc, pacc, kres, qs, vres, dos, C::RES_PLANE, C::TILE_PLANE);
+    scores2_issue<KB>(sacc, pacc, kres, qs, vres, dos, C::RES_PLANE, C::TILE_PLANE);
+    wgmma_wait<0>();
+    acc_fence(sacc);
+    acc_fence(pacc);
     const int qvalid = Lq - it * 64;
     uint32_t pf[4][NS][4], sf[4][NS][4];
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const unsigned long long mb = mrow[i] ? __ldg(mrow[i] + it) : 0ull;
-      const bool valid_row = krow[i] < Lk;
+    for (int c = 0; c < 8; ++c) {   // this thread's query columns c * 8 + 2 * t4 + {0, 1}, both key rows
+      const float4 lq4 = *reinterpret_cast<const float4 *>(qvs + c * 8 + 2 * t4);
+      const float lse2[2] = {lq4.x, lq4.z}, dl[2] = {lq4.y, lq4.w};
+      uint32_t sd[2];
 #pragma unroll
-      for (int c = 0; c < 8; ++c) {
+      for (int e = 0; e < 2; ++e)
+        sd[e] = dropout ? drop_tile_seed(seed, (uint32_t)bh, (uint32_t)(it * 64 + c * 8 + 2 * t4 + e), ktile) : 0u;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const bool valid_row = krow[i] < Lk;
         float pt[2], ds[2];
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int col = c * 8 + 2 * t4 + e;
-          const bool vis = col < qvalid && valid_row && !((mb >> col) & 1ull);
-          const float p = vis ? ex2_approx_b(fmaf(sacc[c * 4 + i * 2 + e], LOG2E, -lse16[c * 2 + e])) : 0.f;
+          const bool vis = col < qvalid && valid_row && !((mb[i] >> col) & 1ull);
+          const float p = vis ? ex2_approx_b(fmaf(sacc[c * 4 + i * 2 + e], LOG2E, -lse2[e])) : 0.f;
           const float dp = pacc[c * 4 + i * 2 + e];
           float m = 1.0f;
-          if (dropout) m = (sd16[c * 2 + e] * ja[i] + jc[i] >= thresh32) ? keep_scale : 0.f;
+          if (dropout) m = (sd[e] * ja[i] + jc[i] >= thresh32) ? keep_scale : 0.f;
           pt[e] = p * m;
-          ds[e] = p * (dp * m - dl16[c * 2 + e]);
+          ds[e] = p * (dp * m - dl[e]);
         }
         uint32_t wp[NS], ws[NS];
         split_pair<NS>(pt[0], pt[1], wp);
@@ -398,8 +430,8 @@ attn_bwd_dkv_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B,
 }
 
 template <int HD>
-int launch_bwd(const BwdMaps &mq, const BwdMaps &mk, int b, int h, int lq, int lk, float scale, const float *lse,
-               const float *delta, float *dq, float *dk, float *dv, long long ld_dq, long long ld_dk, long long ld_dv,
+int launch_bwd(const BwdMaps &mq, const BwdMaps &mk, int b, int h, int lq, int lk, float scale, const float2 *qv,
+               float *dq, float *dk, float *dv, long long ld_dq, long long ld_dk, long long ld_dv,
                const unsigned long long *mask_q, const unsigned long long *mask_k, float dropout_p, unsigned int seed,
                const unsigned int *seed_dev, cudaStream_t s) {
   constexpr int NWG = HD == 64 ? 2 : 1;
@@ -415,9 +447,9 @@ int launch_bwd(const BwdMaps &mq, const BwdMaps &mk, int b, int h, int lq, int l
   }
   const int bh = b * h, rows = 64 * NWG;
   attn_bwd_dq_kernel<HD, NWG><<<dim3((lq + rows - 1) / rows, bh), C::THREADS, C::TOTAL + 1024, s>>>(
-      mq, lq, lk, b, h, scale, lse, delta, dq, ld_dq, mask_q, dropout_p, seed, seed_dev);
+      mq, lq, lk, b, h, scale, qv, dq, ld_dq, mask_q, dropout_p, seed, seed_dev);
   attn_bwd_dkv_kernel<HD, NWG><<<dim3((lk + rows - 1) / rows, bh), C::THREADS, C::TOTAL + 1024, s>>>(
-      mk, lq, lk, b, h, lse, delta, dk, dv, ld_dk, ld_dv, mask_k, dropout_p, seed, seed_dev);
+      mk, lq, lk, b, h, qv, dk, dv, ld_dk, ld_dv, mask_k, dropout_p, seed, seed_dev);
   return launch_status();
 }
 
@@ -427,8 +459,9 @@ extern "C" {
 
 long long coda_attention_bwd_workspace_bytes(int b, int h, int lq, int lk, int hd) {
   const long long bh = (long long)b * h;
-  // q, dO rows; k, v rows (NS bf16 planes each) + delta
-  return 2LL * NS * bh * hd * (2LL * lq + 2LL * lk) + 4LL * bh * lq + 4096;
+  // q, dO rows; k, v rows (NS bf16 planes each) + (lse log2 e, D) per query, padded to whole 64-query tiles
+  const long long lqp = (lq + 63LL) / 64 * 64;
+  return 2LL * NS * bh * hd * (2LL * lq + 2LL * lk) + 8LL * bh * lqp + 4096;
 }
 
 int coda_attention_bwd(int b, int h, int lq, int lk, int hd, float scale, const float *q, const float *k,
@@ -464,7 +497,7 @@ int coda_attention_bwd_ex(int b, int h, int lq, int lk, int hd, float scale, con
   __nv_bfloat16 *dop = w;                                  w += (size_t)NS * bh * lq * hd;
   __nv_bfloat16 *kp = w;                                   w += (size_t)NS * bh * lk * hd;
   __nv_bfloat16 *vp = w;                                   w += (size_t)NS * bh * lk * hd;
-  float *delta = (float *)(((uintptr_t)w + 255) & ~(uintptr_t)255);
+  float2 *qv = (float2 *)(((uintptr_t)w + 255) & ~(uintptr_t)255);
   if ((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)dout) & 15) != 0) return CODA_EINVAL;
   PackJobs jobs = {};
   const long long e = (long long)h * hd;
@@ -474,7 +507,9 @@ int coda_attention_bwd_ex(int b, int h, int lq, int lk, int hd, float scale, con
   jobs.job[3] = {v, vp, lk, 1.0f, ld_v};
   const long long t4 = (long long)(lq > lk ? lq : lk) * bh * hd / 4;
   pack_rows_multi_kernel<NS, false><<<dim3((unsigned)((t4 + 255) / 256), 4), 256, 0, s>>>(jobs, b, h, hd);
-  bwd_delta_kernel<<<(unsigned)(((long long)lq * bh * 32 + 255) / 256), 256, 0, s>>>(lq, b, h, hd, dout, out, delta);
+  const int lqp = (lq + 63) / 64 * 64;
+  bwd_delta_kernel<<<(unsigned)(((long long)lqp * bh * 32 + 255) / 256), 256, 0, s>>>(lq, lqp, b, h, hd, dout, out, lse,
+                                                                                      qv);
   int st = launch_status();
   if (st != CODA_OK) return st;
 
@@ -494,9 +529,9 @@ int coda_attention_bwd_ex(int b, int h, int lq, int lk, int hd, float scale, con
 #undef MAP
   }
   if (hd == 64)
-    return launch_bwd<64>(mq, mk, b, h, lq, lk, scale, lse, delta, dq, dk, dv, ld_dq, ld_dk, ld_dv, mask_q, mask_k,
+    return launch_bwd<64>(mq, mk, b, h, lq, lk, scale, qv, dq, dk, dv, ld_dq, ld_dk, ld_dv, mask_q, mask_k,
                           dropout_p, seed, seed_dev, s);
-  return launch_bwd<128>(mq, mk, b, h, lq, lk, scale, lse, delta, dq, dk, dv, ld_dq, ld_dk, ld_dv, mask_q, mask_k,
+  return launch_bwd<128>(mq, mk, b, h, lq, lk, scale, qv, dq, dk, dv, ld_dq, ld_dk, ld_dv, mask_q, mask_k,
                          dropout_p, seed, seed_dev, s);
 }
 

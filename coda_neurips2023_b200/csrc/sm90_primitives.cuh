@@ -150,6 +150,12 @@ __device__ __forceinline__ void acc_zero(float (&d)[R]) {
 #pragma unroll
   for (int i = 0; i < R; ++i) d[i] = 0.f;
 }
+// Move registers between warpgroups: a TMA-producer warpgroup lowers its per-thread budget so that the MMA
+// warpgroups can raise theirs (every thread of the warpgroup executes the same instruction).  N: 24..256, step 8.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 // named barrier over the first `threads` threads of the CTA (id 0 is __syncthreads)
 __device__ __forceinline__ void bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
