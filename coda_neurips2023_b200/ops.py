@@ -1280,11 +1280,14 @@ class KVBank:
     Autograd wiring: `_KVBankFn` returns a one-element TOKEN; each layer's cross-attention (`_AttentionBank`) takes the
     token as a differentiable input and reads its K / V slice from the bank.  In the backward every attention node
     writes its dK / dV slice into the bank's gradient buffers in place and returns a zero for the token, so autograd
-    runs `_KVBankFn.backward` exactly once, after the last layer that used the bank."""
+    runs `_KVBankFn.backward` exactly once, after the last layer that used the bank.  A layer whose output does not
+    reach the loss runs no attention backward: `written` records the layers that did, and `_KVBankFn.backward` zeroes
+    the column blocks of the others."""
 
     def __init__(self):
         self.k_all = self.v_all = self.dk_all = self.dv_all = None
         self.nlayers = self.e = 0
+        self.written = set()
 
 
 class _KVBankFn(torch.autograd.Function):
@@ -1305,6 +1308,7 @@ class _KVBankFn(torch.autograd.Function):
         bank.v_all = gemm_a32(xv, pv, nl * e, bias=torch.cat([t.detach() for t in bv]))
         bank.nlayers, bank.e = nl, e
         bank.dk_all = bank.dv_all = None
+        bank.written = set()
         ctx.bank, ctx.nsplit, ctx.shape = bank, nsplit, (lk, b, e)
         ctx.save_for_backward(xk, xv, pk, pv, *params)
         return torch.zeros(1, dtype=torch.float32, device=memory.device)
@@ -1318,6 +1322,10 @@ class _KVBankFn(torch.autograd.Function):
         nl = bank.nlayers
         dk_all, dv_all = bank.dk_all, bank.dv_all
         assert dk_all is not None and dv_all is not None, "no cross-attention used the K / V bank"
+        for i in range(nl):
+            if i not in bank.written:      # this layer's output did not reach the loss: its dK / dV are zero
+                dk_all[:, i * e: (i + 1) * e].zero_()
+                dv_all[:, i * e: (i + 1) * e].zero_()
         ns = min(ctx.nsplit, BACKWARD_NSPLIT)
         d_key = d_mem = None
         if ctx.needs_input_grad[0]:
@@ -1334,6 +1342,7 @@ class _KVBankFn(torch.autograd.Function):
                 dw = gemm_tn32(dy, x, out=sw, colsum_out=db)
                 grads += [dw if sw is None else _sunk(sw), db if sb is None else _sunk(sb)]
         bank.k_all = bank.v_all = bank.dk_all = bank.dv_all = None
+        bank.written = set()
         return (d_key, d_mem, None, None, *grads)
 
 
@@ -1359,13 +1368,14 @@ class _AttentionBank(torch.autograd.Function):
         q, k, v, out, lse = ctx.saved_tensors
         bank, idx, e = ctx.bank, ctx.idx, ctx.bank.e
         lk, b, _ = k.shape
-        if bank.dk_all is None:          # every layer writes its own column block completely: no zero fill
+        if bank.dk_all is None:          # a layer that runs this backward writes its whole block: no zero fill
             bank.dk_all = torch.empty((lk * b, bank.nlayers * e), dtype=torch.float32, device=q.device)
             bank.dv_all = torch.empty((lk * b, bank.nlayers * e), dtype=torch.float32, device=q.device)
         dk = bank.dk_all.view(lk, b, -1)[..., idx * e: (idx + 1) * e]
         dv = bank.dv_all.view(lk, b, -1)[..., idx * e: (idx + 1) * e]
         dq = torch.empty(q.shape, dtype=torch.float32, device=q.device)
         attention_launch.backward(q, k, v, out, dout, lse, ctx.nhead, ctx.dropout_p, ctx.salt, grads=(dq, dk, dv))
+        bank.written.add(idx)
         return dq, torch.zeros(1, dtype=torch.float32, device=q.device), None, None, None, None, None
 
 

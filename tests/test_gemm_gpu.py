@@ -168,3 +168,112 @@ def test_fp16_linear_with_fused_residual_and_gelu():
     # 3-D input / residual (L, N, D) as the tower passes them
     x3, r3 = x.view(50, 6, k), res.view(50, 6, n)
     assert torch.equal(ops.linear(x3, w, b, residual=r3).view(m, n), ops.linear(x, w, b, residual=res))
+
+
+# ---------------------------------------------------------------- every instance, tile edges, split-K epilogue
+# (nsplit, fp16, batch, m, n, k, bias, relu, ldc_pad): tests/test_gemm_instances_cpu.py checks that these reach every
+# instance coda_gemm_nt can select and both sides of its split-K rule.  Output rows are ldc = n + ldc_pad apart.
+NT_CASES = [
+    # m, n, k at 1 and on either side of 64 and 128, on every fp32-plane instance
+    (1, False, 1, 1, 1, 1, True, False, 0),
+    (2, False, 1, 63, 65, 64, True, False, 3),
+    (3, False, 1, 64, 63, 65, False, True, 0),
+    (1, False, 1, 65, 64, 63, True, True, 1),
+    (2, False, 1, 127, 129, 128, False, False, 4),
+    (3, False, 1, 128, 127, 129, True, False, 0),
+    (1, False, 1, 129, 128, 127, False, False, 2),
+    (2, False, 1, 1, 64, 129, True, True, 0),
+    (3, False, 1, 129, 1, 1, True, False, 5),
+    # fp16 operands: 64-, 128-, 192- and 256-wide tiles, n = 512 below the 256-wide threshold
+    (1, True, 1, 65, 1, 64, True, False, 0),
+    (1, True, 1, 64, 64, 127, True, True, 3),
+    (1, True, 1, 129, 65, 128, True, False, 0),
+    (1, True, 1, 300, 512, 192, True, False, 4),
+    (1, True, 1, 100, 1000, 64, False, False, 0),
+    (1, True, 1, 200, 384, 64, True, False, 0),
+    (1, True, 1, 130, 1536, 128, True, True, 0),
+    # split-K: the bias, the batch index and ldc > n are handled by splitk_reduce_kernel, not the GEMM epilogue
+    (1, False, 2, 129, 65, 4096, True, False, 3),
+    (2, False, 3, 100, 64, 2100, True, False, 4),
+    (3, False, 1, 200, 300, 8192, True, False, 0),
+    (1, True, 2, 64, 200, 4096, True, False, 8),
+    # a long contraction with ReLU never splits
+    (2, False, 1, 100, 64, 4096, True, True, 0),
+]
+
+# exact fp16 operands: only the fp32 accumulation errs, as with three planes
+FP16_TOL = TOL[3]
+SENTINEL = 1234.5
+
+
+def _nt_operand(x, nsplit, fp16):
+    """(batch, rows, k) fp32 -> planes (nsplit, batch, rows, kpad): split bf16 planes, or one zero-padded fp16 plane"""
+    batch, rows, k = x.shape
+    if fp16:
+        p = torch.zeros(1, batch, rows, ops._pad64(k), dtype=torch.float16, device=x.device)
+        p[0, :, :, :k] = x.half()
+        return p
+    return ops.pack_split(x, rows, k, k, 1, nsplit, batch=batch, batch_stride=rows * k)
+
+
+@pytest.mark.parametrize("nsplit,fp16,batch,m,n,k,bias,relu,ldc_pad", NT_CASES)
+def test_gemm_nt_instances_and_edges_vs_fp64(nsplit, fp16, batch, m, n, k, bias, relu, ldc_pad):
+    torch.manual_seed(7 * m + 3 * n + k + batch)
+    a = torch.randn(batch, m, k, device="cuda")
+    b = torch.randn(batch if batch == 3 else 1, n, k, device="cuda")      # batch 3: per-entry B, else shared weights
+    if fp16:
+        a, b = a.half().float(), b.half().float()
+    bvec = torch.randn(n, device="cuda") if bias else None
+    ap, bp = _nt_operand(a, nsplit, fp16), _nt_operand(b, nsplit, fp16)
+    full = torch.full((batch, m, n + ldc_pad), SENTINEL, device="cuda")
+    c = ops.gemm_nt(ap, bp, m, n, bias=bvec, relu=relu, out=full[..., :n])
+    ref = _ref(a, b, bvec, relu)
+    scale = (a.double().abs() @ b.double().abs().transpose(-1, -2)).max()
+    err = ((c.double() - ref).abs().max() / scale).item()
+    assert err < (FP16_TOL if fp16 else TOL[nsplit]), f"err {err:.2e}"
+    assert bool((full[..., n:] == SENTINEL).all()), "a column >= n of the strided output was written"
+    again = ops.gemm_nt(ap, bp, m, n, bias=bvec, relu=relu)
+    assert torch.equal(again, c)
+
+
+# (nsplit, mc, m, n): C (m, n) = A^T B over mc rows.  The 2- and 3-row outputs are the prediction heads' weight
+# gradients (n_out = 2 / 3 rows, one per output feature), which run here on two planes.
+TN_CASES = [
+    (1, 1, 64, 64),
+    (1, 65, 130, 129),
+    (2, 1, 3, 2),
+    (2, 65, 2, 256),
+    (2, 4100, 3, 256),
+    (2, 4100, 128, 3),
+    (2, 3000, 130, 200),
+    (2, 200000, 64, 64),
+    (3, 65, 63, 65),
+    (3, 200000, 128, 48),
+]
+
+
+def _tn(nsplit, mc, m, n, seed):
+    torch.manual_seed(seed)
+    a = torch.randn(mc, m, device="cuda")
+    b = torch.randn(mc, n, device="cuda")
+    return a, b, ops.pack_split(a, mc, m, m, 1, nsplit), ops.pack_split(b, mc, n, n, 1, nsplit)
+
+
+@pytest.mark.parametrize("nsplit,mc,m,n", TN_CASES)
+def test_gemm_tn_instances_and_edges_vs_fp64(nsplit, mc, m, n):
+    a, b, ap, bp = _tn(nsplit, mc, m, n, mc + 5 * m + n)
+    c = ops.gemm_tn(ap, bp, m, n)
+    ref = a.double().t() @ b.double()
+    scale = (a.double().abs().t() @ b.double().abs()).max()
+    err = ((c.double() - ref).abs().max() / scale).item()
+    assert err < TOL[nsplit], f"err {err:.2e}"
+
+
+def test_gemm_tn_same_bits_after_a_larger_split_k_launch():
+    """The heads' weight-gradient shape splits K; a larger split-K launch in between leaves its partial tiles in the
+    shared scratch.  The second call must give the same bits."""
+    _, _, ap, bp = _tn(2, 4100, 3, 256, 11)
+    c1 = ops.gemm_tn(ap, bp, 3, 256)
+    _, _, bigp, bigq = _tn(2, 200000, 256, 128, 12)
+    ops.gemm_tn(bigp, bigq, 256, 128)
+    assert torch.equal(ops.gemm_tn(ap, bp, 3, 256), c1)
