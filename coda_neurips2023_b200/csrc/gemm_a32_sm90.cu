@@ -90,10 +90,11 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
   const bool two_in = P.mode == CODA_A32_BN_BWD;
   const bool pooled = P.mode == CODA_A32_BN_BWD_POOLED || P.mode == CODA_A32_BN_BWD_POOLED_PRE;
   // pooled BatchNorm backward: each raw stage carries, after the fp32 tile, the (group, channel) gradient and
-  // arg-max rows of the tile's groups for this k-block: [groups in tile][64 floats | 64 bytes]  (<= 1 KB)
-  const int raw_stage_bytes = RAW_TILE * (two_in ? 2 : 1) + (pooled ? 1024 : 0);
-  const uint32_t nraw = (uint32_t)((RAW_KB * 1024) / raw_stage_bytes);
+  // arg-max rows of the tile's groups for this k-block: [groups in tile][64 floats | 64 bytes], rounded up to whole
+  // KB so that the next stage's TMA boxes stay 1024-byte aligned (groups of 32 rows: four groups, 1280 bytes)
   const int tile_groups = pooled ? (P.group >= BM ? 1 : BM / P.group) : 0;
+  const int raw_stage_bytes = RAW_TILE * (two_in ? 2 : 1) + (tile_groups * 320 + 1023) / 1024 * 1024;
+  const uint32_t nraw = (uint32_t)((RAW_KB * 1024) / raw_stage_bytes);
   unsigned char *b_ring = smem + (size_t)RAW_KB * 1024;
   float *s_stats = reinterpret_cast<float *>(b_ring + (size_t)B_STAGES * B_STAGE);   // [8 warps][2][n] (only if P.stats)
   __shared__ __align__(8) uint64_t raw_full[MAX_RAW], raw_empty[MAX_RAW];

@@ -49,6 +49,10 @@ def applicable(x: torch.Tensor, blocks, group: int) -> bool:
             return False
         if li < len(blocks) - 1 and cout % 64 != 0:
             return False
+        if cout > 256 and (li > 0 or cin > 8):
+            # a GEMM layer's column statistics (16 x cout floats) share the fp32-A GEMM's shared memory with its
+            # stages: every instance fits them up to 256 columns (launch_a32 in gemm_a32_sm90.cu)
+            return False
     return True
 
 

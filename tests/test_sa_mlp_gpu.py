@@ -75,3 +75,15 @@ def test_fused_path_declines_what_it_does_not_cover():
     with torch.no_grad():
         assert mlp.forward_max_pooled(x) is None                        # inference
     assert pt_utils.SharedMLP([3, 64, 128], bn=False).cuda().forward_max_pooled(x) is None   # conv bias, no bn
+    # the tiny-K first layer produces no input gradient
+    assert mlp.forward_max_pooled(x.clone().requires_grad_(True)) is None
+    # cin > 8 and not a multiple of 64; a non-last width that is not a multiple of 64; a group of more than 256 rows
+    assert pt_utils.SharedMLP([72, 64], bn=True).cuda().forward_max_pooled(torch.randn(1, 72, 4, 8, device="cuda")) \
+        is None
+    assert pt_utils.SharedMLP([64, 96, 128], bn=True).cuda().forward_max_pooled(
+        torch.randn(1, 64, 4, 8, device="cuda")) is None
+    assert mlp.forward_max_pooled(torch.randn(1, 3, 2, 257, device="cuda")) is None
+    # GEMM layers wider than 256 columns: the GEMM's column statistics would not fit in its shared memory
+    assert pt_utils.SharedMLP([64, 512, 1024], bn=True).cuda().forward_max_pooled(
+        torch.randn(1, 64, 4, 32, device="cuda")) is None
+    assert mlp.forward_max_pooled(torch.randn(1, 3, 2, 256, device="cuda")) is not None
