@@ -156,11 +156,12 @@ def _lcg_jump():
     return ja, jc
 
 
-def dropout_keep(bh: int, lq: int, lk: int, dropout_p: float, salt: int, device) -> torch.Tensor:
-    """(bh, lq, lk) bool keep-mask, bit-identical to drop_keep() in csrc/attention_common.cuh."""
+def dropout_keep(bh: int, lq: int, lk: int, dropout_p: float, salt: int, device, bh0: int = 0) -> torch.Tensor:
+    """(bh, lq, lk) bool keep-mask of the (batch * head) rows bh0 .. bh0 + bh - 1, bit-identical to drop_keep() in
+    csrc/attention_common.cuh."""
     M = 0xFFFFFFFF
     seed = (seed_counter(device).to(torch.int64) & M) + (salt & M)   # stays on the device: no sync
-    ib = torch.arange(bh, device=device, dtype=torch.int64).view(bh, 1, 1)
+    ib = torch.arange(bh0, bh0 + bh, device=device, dtype=torch.int64).view(bh, 1, 1)
     iq = torch.arange(lq, device=device, dtype=torch.int64).view(1, lq, 1)
     ik = torch.arange(lk, device=device, dtype=torch.int64).view(1, 1, lk)
     h = (seed + ib * 0x9E3779B1 + iq * 0x85EBCA77 + (ik >> 6) * 0xC2B2AE3D) & M   # one hash per 64-key tile

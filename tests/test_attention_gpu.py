@@ -23,7 +23,10 @@ CASES = [
 ]
 
 
-@pytest.mark.parametrize("nsplit,tol", [(3, 5e-6), (2, 1e-4), (1, 2e-2)])
+NSPLIT_TOLS = [(3, 5e-6), (2, 1e-4), (1, 2e-2)]
+
+
+@pytest.mark.parametrize("nsplit,tol", NSPLIT_TOLS)
 @pytest.mark.parametrize("lq,lk,b,h,hd", CASES)
 def test_attention_forward_vs_fp64(lq, lk, b, h, hd, nsplit, tol):
     torch.manual_seed(lq + lk + hd)
@@ -71,9 +74,12 @@ def test_attention_autograd_wrapper():
     assert (outs.mean(0) - ref.detach()).abs().mean().item() < 0.05
 
 
-@pytest.mark.parametrize("lq,lk,b,h,hd", [
+BWD_CASES = [
     (128, 128, 1, 1, 64), (2048, 2048, 1, 4, 64), (300, 200, 2, 2, 64), (64, 1000, 2, 4, 64), (50, 50, 3, 12, 64),
-    (128, 64, 1, 1, 128), (256, 2048, 2, 4, 128), (256, 256, 2, 4, 128), (130, 200, 1, 2, 128), (3, 2, 1, 1, 128)])
+    (128, 64, 1, 1, 128), (256, 2048, 2, 4, 128), (256, 256, 2, 4, 128), (130, 200, 1, 2, 128), (3, 2, 1, 1, 128)]
+
+
+@pytest.mark.parametrize("lq,lk,b,h,hd", BWD_CASES)
 @pytest.mark.parametrize("p", [0.0, 0.1])
 def test_attention_backward_vs_fp64(lq, lk, b, h, hd, p):
     torch.manual_seed(lq + lk)
@@ -117,8 +123,11 @@ def test_attention_forward_reads_fp16_slices_of_a_fused_projection_in_place():
     assert torch.equal(o_s, o_c)
 
 
-@pytest.mark.parametrize("lq,lk,b,h,hd", [(256, 256, 2, 4, 64), (2048, 2048, 1, 4, 64), (130, 200, 2, 2, 64),
-                                          (256, 2048, 2, 4, 128), (100, 77, 1, 2, 128)])
+MASKED_CASES = [(256, 256, 2, 4, 64), (2048, 2048, 1, 4, 64), (130, 200, 2, 2, 64), (256, 2048, 2, 4, 128),
+                (100, 77, 1, 2, 128)]
+
+
+@pytest.mark.parametrize("lq,lk,b,h,hd", MASKED_CASES)
 @pytest.mark.parametrize("p", [0.0, 0.1])
 def test_masked_attention_forward_backward_vs_fp64(lq, lk, b, h, hd, p):
     """Boolean attn_mask (True = not visible; nn.MultiheadAttention's convention, the reference's masked encoder
