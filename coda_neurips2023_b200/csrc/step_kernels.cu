@@ -477,7 +477,9 @@ int coda_masked_l1_fwd(int layers, long long rows, int d, const float *pred, con
                        float *out, float *scratch, void *stream) {
   if (layers < 0 || rows < 0 || d <= 0 || (d & 3)) return CODA_EINVAL;
   if (layers == 0) return CODA_OK;
-  if (!pred || !target || !w || !out || !scratch || (((uintptr_t)pred | (uintptr_t)target) & 15)) return CODA_EINVAL;
+  // with no rows the operands are empty (and may be NULL): every out[l] is 0
+  if ((rows > 0 && (!pred || !target || !w)) || !out || !scratch || (((uintptr_t)pred | (uintptr_t)target) & 15))
+    return CODA_EINVAL;
   cudaStream_t s = (cudaStream_t)stream;
   masked_l1_fwd_kernel<<<dim3(L1_BLOCKS, layers), THREADS, 0, s>>>(rows, d, pred, target, w, scratch);
   int st = coda::launch_status();

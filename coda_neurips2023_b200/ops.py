@@ -344,6 +344,9 @@ def sum_tensors(ts, out: torch.Tensor | None = None) -> torch.Tensor:
     if out is None:
         out = torch.empty_like(ts[0])
     assert out.is_contiguous() and all(t.shape == ts[0].shape for t in ts)
+    if any(t.data_ptr() == out.data_ptr() for t in ts[_SUM_MAX:]):
+        # the first pass would overwrite an operand of a later pass before that pass reads it
+        return sum_tensors([sum_tensors(ts)], out=out)
     n = ts[0].numel()
     with torch.cuda.device(out.device):
         while True:

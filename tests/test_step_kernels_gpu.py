@@ -109,7 +109,8 @@ def test_flat_adamw_matches_torch_adamw_with_clip(filter_biases):
     from coda_neurips2023_b200.engine import FlatAdamW, FlatParameters, _no_decay
 
     torch.manual_seed(3)
-    # odd sizes: chunks start at offsets that are not multiples of 4, one tensor longer than a chunk
+    # odd sizes and one tensor longer than a chunk; FlatParameters starts every tensor on a 64-element boundary, so
+    # the chunk offsets are multiples of 4 here (test_step_glue_edges_gpu.py runs unaligned chunk tables)
     model = torch.nn.Sequential(torch.nn.Linear(37, 501), torch.nn.ReLU(), torch.nn.Linear(501, 129),
                                 torch.nn.LayerNorm(129), torch.nn.Linear(129, 7)).cuda()
     ref = copy.deepcopy(model)
