@@ -131,6 +131,8 @@ class PointnetSAModuleVotes(nn.Module):
             grouped_features, grouped_xyz, unique_cnt = self.grouper(xyz, new_xyz, features)
 
         new_features = self.mlp_module.forward_max_pooled(grouped_features) if self.pooling == "max" else None
+        if new_features is None and self.pooling == "max":
+            new_features = self.mlp_module.forward_max_pooled_infer(grouped_features)   # eval mode, no autograd
         if new_features is None:
             new_features = self.mlp_module(grouped_features)  # (B, mlp[-1], npoint, nsample)
             new_features = _pool_over_samples(new_features, self.pooling, grouped_xyz, self.sigma, self.nsample)

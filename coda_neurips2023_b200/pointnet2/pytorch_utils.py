@@ -157,6 +157,30 @@ class SharedMLP(nn.Sequential):
         pooled = sa_mlp.shared_mlp_max(rows, blocks, s)          # (B * npoint, C_out)
         return pooled.view(b, p, -1).permute(0, 2, 1)
 
+    def forward_max_pooled_infer(self, x):
+        """Inference form of forward_max_pooled (eval-mode BatchNorm with running statistics, nothing for autograd
+        to record): the whole MLP + max over nsample as one kernel (sa_mlp.shared_mlp_max_infer) that reads the
+        grouped (B, C, npoint, nsample) map in place -> (B, C_out, npoint).  Returns None when it does not apply
+        (training-mode BatchNorm, gradients wanted, a layout other than the pre-encoder's); the caller then runs
+        forward() and pools itself."""
+        from .. import sa_mlp
+
+        if x.dim() != 4 or not x.is_cuda:
+            return None
+        blocks = []
+        for block in self:
+            mods = list(block.children())
+            if (len(mods) != 3 or not isinstance(mods[0], nn.Conv2d) or mods[0].kernel_size != (1, 1)
+                    or not isinstance(mods[1], _NormWrap) or not isinstance(mods[1][0], nn.BatchNorm2d)
+                    or not isinstance(mods[2], nn.ReLU)):
+                return None
+            blocks.append((mods[0], mods[1][0]))
+        b, _, p, s = x.shape
+        if not sa_mlp.infer_applicable(x, blocks, s):
+            return None
+        pooled = sa_mlp.shared_mlp_max_infer(x, blocks, s)       # (B * npoint, C_out)
+        return pooled.view(b, p, -1).permute(0, 2, 1)
+
     def __init__(self, args: List[int], *, bn: bool = False, activation=nn.ReLU(inplace=True),
                  preact: bool = False, first: bool = False, name: str = ""):
         super().__init__()

@@ -15,6 +15,10 @@ ReLU blocks) followed by the `F.max_pool2d(kernel_size=[1, nsample])` of `Pointn
 
 Kernels: csrc/sa_mlp_kernels.cu (include/coda_sa_mlp.h).  There is no CPU / eager fallback in here: callers
 (`SharedMLP.forward_max_pooled`) check `applicable()` first and use the module-by-module path otherwise.
+
+Inference (eval-mode BatchNorm, nothing for autograd to record): `shared_mlp_max_infer` runs the pre-encoder's
+whole 3 -> 64 -> 128 -> 256 MLP + max as one kernel (csrc/sa_infer_sm90.cu) that writes only the pooled rows;
+`SharedMLP.forward_max_pooled_infer` checks `infer_applicable()` first.
 """
 from __future__ import annotations
 
@@ -297,3 +301,63 @@ def shared_mlp_max(x_rows: torch.Tensor, blocks, group: int, nsplit: int | None 
     pooled, _ = _SharedMLPMax.apply(x_rows.contiguous(), int(group), ops.DEFAULT_NSPLIT if nsplit is None else nsplit,
                                     [bn for _, bn in blocks], *params)
     return pooled
+
+
+# --------------------------------------------------------------------------- inference (eval-mode BatchNorm)
+# The one layout the inference kernel covers (csrc/sa_infer_sm90.cu): the 3DETR pre-encoder, xyz (+ rgb) input.
+INFER_WIDTHS = (64, 128, 256)
+INFER_GROUP = 64
+
+
+def infer_applicable(x: torch.Tensor, blocks, group: int) -> bool:
+    """Can the inference kernel compute `blocks` + max over `group` on x (B, C0, npoint, nsample)?  Only with every
+    BatchNorm in eval mode with running statistics, and only when autograd would record nothing."""
+    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and group == INFER_GROUP
+            and x.shape[3] == group and x.shape[1] in (3, 6) and len(blocks) == len(INFER_WIDTHS)):
+        return False
+    if x.stride(3) != 1:
+        return False
+    params = [t for conv, bn in blocks for t in (conv.weight, bn.weight, bn.bias)]
+    if torch.is_grad_enabled() and (x.requires_grad or any(p is not None and p.requires_grad for p in params)):
+        return False
+    cin = x.shape[1]
+    for (conv, bn), cout in zip(blocks, INFER_WIDTHS):
+        if conv.bias is not None or tuple(conv.weight.shape) != (cout, cin, 1, 1):
+            return False
+        if bn.training or not bn.affine or bn.running_mean is None or bn.running_var is None:
+            return False
+        if any(t.dtype != torch.float32 or t.device != x.device
+               for t in (conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var)):
+            return False
+        cin = cout
+    return True
+
+
+def _folded_affine(blocks) -> torch.Tensor:
+    """[scale1 | shift1 | scale2 | shift2 | scale3 | shift3] of the eval-mode BatchNorms, from the current running
+    statistics (recomputed every call: a changed statistic is never stale)."""
+    parts = []
+    with torch.no_grad():
+        for _, bn in blocks:
+            scale = bn.weight * torch.rsqrt(bn.running_var + bn.eps)
+            parts += [scale, bn.bias - bn.running_mean * scale]
+        return torch.cat(parts)
+
+
+def shared_mlp_max_infer(x: torch.Tensor, blocks, group: int) -> torch.Tensor:
+    """x (B, C0, npoint, nsample) grouped features, read in place -> (B * npoint, 256): max over the neighbours of
+    relu(bn(conv(...))) with eval-mode BatchNorm, in one kernel.  Call infer_applicable() first."""
+    b, c0, npoint, nsample = x.shape
+    (conv1, _), (conv2, _), (conv3, _) = blocks
+    w1 = conv1.weight.detach().reshape(INFER_WIDTHS[0], c0).contiguous()
+    w2 = ops._packed_weight(conv2.weight.reshape(INFER_WIDTHS[1], -1), False, ops.DEFAULT_NSPLIT)
+    w3 = ops._packed_weight(conv3.weight.reshape(INFER_WIDTHS[2], -1), False, ops.DEFAULT_NSPLIT)
+    affine = _folded_affine(blocks)
+    out = torch.empty((b * npoint, INFER_WIDTHS[2]), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        st = lib().coda_sa_mlp_max_infer(_ll(b), _i(c0), _i(npoint), _i(nsample), ptr(x), _ll(x.stride(0)),
+                                         _ll(x.stride(1)), _ll(x.stride(2)), ptr(w1), ptr(w2), _ll(w2.stride(0)),
+                                         ptr(w3), _ll(w3.stride(0)), ptr(affine), ptr(out), _ll(out.stride(0)),
+                                         stream_of(x))
+    check(st, "sa_mlp_max_infer")
+    return out

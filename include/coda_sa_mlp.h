@@ -141,6 +141,25 @@ int coda_bn_relu_bwd_small_k(long long rows, int cin, int cout, const float *y, 
                              const float *invstd, const float *gamma, const float *beta, const float *s1,
                              const float *s2, const float *x, float *dw, float *scratch, void *stream);
 
+/*
+ * Inference (eval-mode BatchNorm) form of the pre-encoder's whole shared MLP + max over neighbours, one kernel
+ * (csrc/sa_infer_sm90.cu):
+ *   out[b * npoint + p][:] = max_j relu(A3(W3 relu(A2(W2 relu(A1(W1 x[b, :, p, j]))))))
+ * with A_l(v) = v * scale_l + shift_l the folded running-statistics BatchNorm of layer l.
+ *   x        grouped input (batch, c0, npoint, nsample), element strides x_*_stride, neighbour stride 1;
+ *            c0 in {3, 6}, nsample == 64
+ *   w1       (64, c0) fp32
+ *   w2_planes bf16 planes [3][128][64] (plane stride in elements), W2 (128, 64) as packed by
+ *            coda_pack_split_bf16_strided; w3_planes: the same for W3 (256, 128), of which planes 0 and 1 are read
+ *   affine   fp32 [scale1 (64) | shift1 (64) | scale2 (128) | shift2 (128) | scale3 (256) | shift3 (256)]
+ *   out      (batch * npoint, 256) fp32, row stride ldo >= 256
+ * Other layouts return CODA_EINVAL.  Deterministic (no atomics).
+ */
+int coda_sa_mlp_max_infer(long long batch, int c0, int npoint, int nsample, const float *x, long long x_batch_stride,
+                          long long x_channel_stride, long long x_point_stride, const float *w1, const void *w2_planes,
+                          long long w2_plane_stride, const void *w3_planes, long long w3_plane_stride,
+                          const float *affine, float *out, long long ldo, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
