@@ -16,7 +16,9 @@
 // Warp roles (288 threads, persistent CTAs, one per SM):
 //   warp 8      TMA producer: raw fp32 A boxes -> raw ring, B plane boxes -> B ring
 //   warps 0-7   two consumer warpgroups (rows [0, 64) and [64, 128) of the tile): prologue -> register A
-//               fragments -> wgmma.mma_async (B from shared memory) -> register accumulators -> epilogue
+//               fragments -> wgmma.mma_async (B from shared memory) -> register accumulators -> epilogue.
+//               Named barriers make them issue each k-block's wgmmas in turn, so that one converts while the
+//               tensor pipe works for the other.
 // C-ABI in include/coda_gemm.h (coda_gemm_a32*).
 #include "../../include/coda_gemm.h"
 #include "sm90_primitives.cuh"
@@ -74,6 +76,24 @@ struct A32Params {
   long long ldc;
   float *stats;            // [gridDim.x][2][n] or null
   int b_resident;          // the whole B operand of this CTA's n-tile stays in shared memory (short contractions)
+};
+
+// Strict alternation of one phase of the two consumer warpgroups: warpgroup 0's i-th phase, then warpgroup 1's
+// i-th, then warpgroup 0's (i+1)-th, ...  Both run the same number of phases.  Warpgroup wg waits on named barrier
+// 2 + wg; the other warpgroup arrives there when its phase ends.  finish() takes warpgroup 1's last arrival.
+struct Alternation {
+  int wg;
+  bool started;
+  __device__ __forceinline__ void begin() {
+    if (wg == 1 || started) bar_sync(2 + wg, 256);
+  }
+  __device__ __forceinline__ void end() {
+    bar_arrive(2 + (wg ^ 1), 256);
+    started = true;
+  }
+  __device__ __forceinline__ void finish() {
+    if (wg == 0 && started) bar_sync(2, 256);
+  }
 };
 
 // RAW_KB: size of the raw-fp32 staging region; it holds RAW_KB / 32 stages (one-input prologues) or RAW_KB / 64
@@ -203,6 +223,11 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
   float acc[BN / 2];
   uint32_t it = 0;
   int m0, n0;
+  // The two warpgroups issue their wgmmas of a k-block in turn, warpgroup 0 first: warpgroup 1's wgmmas queue behind
+  // warpgroup 0's, so warpgroup 0 converts the next k-block (or runs its epilogue) while the tensor pipe still works
+  // for warpgroup 1, and the other way round.  Without the turns both wait on the same stages and convert at the
+  // same time, with the pipe idle.
+  Alternation mma_turn{wg, false};
   for (long long t = 0; tile_at(t, m0, n0); ++t) {
     // pooled mode: the 16 rows of a warp lie in one group (group % 32 == 0); index of each row within it
     int pgt = 0, pgi[2] = {0, 0};
@@ -222,61 +247,83 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
 #pragma unroll
       for (int kk = 0; kk < BK / 16; ++kk) {
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int row = rloc[q & 1];
-          const int col = kk * 16 + (q >> 1) * 8 + 2 * t4;   // column of the k-block (even)
-          const uint32_t off = (uint32_t)(col >> 5) * (RAW_TILE / 2) + (uint32_t)row * 128u +
-                               ((uint32_t)(((col & 31) >> 2) ^ (row & 7)) << 4) + (uint32_t)(col & 3) * 4u;
-          float2 x = *reinterpret_cast<const float2 *>(rt + off);
+        for (int c2 = 0; c2 < 2; ++c2) {
+          // registers q = 2 c2 + i, i = 0, 1 (rows rloc[i]) share their columns and so the per-column operands of the
+          // prologue: those are read once for both rows
+          const int col = kk * 16 + c2 * 8 + 2 * t4;   // column of the k-block (even)
           const int kc = k0 + col;
+          auto off = [&](int i) {
+            const int row = rloc[i];
+            return (uint32_t)(col >> 5) * (RAW_TILE / 2) + (uint32_t)row * 128u +
+                   ((uint32_t)(((col & 31) >> 2) ^ (row & 7)) << 4) + (uint32_t)(col & 3) * 4u;
+          };
+          auto put = [&](int i, float2 x) {
+            uint32_t w[NSPLIT];
+            split_pair<NSPLIT>(x.x, x.y, w);
+#pragma unroll
+            for (int pl = 0; pl < NSPLIT; ++pl) af[kk][pl][c2 * 2 + i] = w[pl];
+          };
+          auto ld2 = [&](const float *v) { return __ldg(reinterpret_cast<const float2 *>(v + kc)); };
           if (P.mode == CODA_A32_AFFINE_RELU) {
-            const float2 s2 = __ldg(reinterpret_cast<const float2 *>(P.scale + kc));
-            const float2 h2 = __ldg(reinterpret_cast<const float2 *>(P.shift + kc));
-            x.x = fmaxf(fmaf(x.x, s2.x, h2.x), 0.f);
-            x.y = fmaxf(fmaf(x.y, s2.y, h2.y), 0.f);
+            const float2 s2 = ld2(P.scale), h2 = ld2(P.shift);
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
+              x.x = fmaxf(fmaf(x.x, s2.x, h2.x), 0.f);
+              x.y = fmaxf(fmaf(x.y, s2.y, h2.y), 0.f);
+              put(i, x);
+            }
           } else if (P.mode == CODA_A32_BN_BWD) {
             // x = y (pre-BN activation), d = gradient of relu(bn(y)).  With s = gamma * invstd, t = beta_bn - mean * s:
             //   dy = s * ([s y + t > 0] d - s1/N - xhat s2/N) = [s y + t > 0] * s * d + alpha * y + beta
             //   alpha = -s * invstd * s2 / N,  beta = -s * s1 / N - alpha * mean        (host: coda_bn_bwd_coefs)
-            const float2 d = *reinterpret_cast<const float2 *>(rt + RAW_TILE + off);
-            const float2 s2 = __ldg(reinterpret_cast<const float2 *>(P.scale + kc));
-            const float2 h2 = __ldg(reinterpret_cast<const float2 *>(P.shift + kc));
-            const float2 a2 = __ldg(reinterpret_cast<const float2 *>(P.alpha + kc));
-            const float2 b2 = __ldg(reinterpret_cast<const float2 *>(P.beta + kc));
-            x.x = (fmaf(x.x, s2.x, h2.x) > 0.f ? s2.x * d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
-            x.y = (fmaf(x.y, s2.y, h2.y) > 0.f ? s2.y * d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
+            const float2 s2 = ld2(P.scale), h2 = ld2(P.shift), a2 = ld2(P.alpha), b2 = ld2(P.beta);
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
+              const float2 d = *reinterpret_cast<const float2 *>(rt + RAW_TILE + off(i));
+              x.x = (fmaf(x.x, s2.x, h2.x) > 0.f ? s2.x * d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
+              x.y = (fmaf(x.y, s2.y, h2.y) > 0.f ? s2.y * d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
+              put(i, x);
+            }
           } else if (P.mode == CODA_A32_BN_BWD_POOLED_PRE) {
             // pre-masked, pre-scaled pooled gradient: one compare + select + FMA + add per element
             const unsigned char *px = rt + RAW_TILE + pgt * 320;
-            const float2 a2 = __ldg(reinterpret_cast<const float2 *>(P.alpha + kc));
-            const float2 b2 = __ldg(reinterpret_cast<const float2 *>(P.beta + kc));
+            const float2 a2 = ld2(P.alpha), b2 = ld2(P.beta);
             const float2 d = *reinterpret_cast<const float2 *>(px + col * 4);
             const uchar2 id = *reinterpret_cast<const uchar2 *>(px + 256 + col);
-            const int gi = pgi[q & 1];
-            x.x = (id.x == gi ? d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
-            x.y = (id.y == gi ? d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
+              const int gi = pgi[i];
+              x.x = (id.x == gi ? d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
+              x.y = (id.y == gi ? d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
+              put(i, x);
+            }
           } else if (P.mode == CODA_A32_BN_BWD_POOLED) {
             // the layer output was max-pooled over `group` rows: only the arg-max row of a (group, channel)
             // carries the incoming gradient dpooled[g][c]
             const unsigned char *px = rt + RAW_TILE + pgt * 320;     // staged by the producer with the raw tile
-            const float2 s2 = __ldg(reinterpret_cast<const float2 *>(P.scale + kc));
-            const float2 h2 = __ldg(reinterpret_cast<const float2 *>(P.shift + kc));
-            const float2 a2 = __ldg(reinterpret_cast<const float2 *>(P.alpha + kc));
-            const float2 b2 = __ldg(reinterpret_cast<const float2 *>(P.beta + kc));
+            const float2 s2 = ld2(P.scale), h2 = ld2(P.shift), a2 = ld2(P.alpha), b2 = ld2(P.beta);
             const float2 d = *reinterpret_cast<const float2 *>(px + col * 4);
             const uchar2 id = *reinterpret_cast<const uchar2 *>(px + 256 + col);
-            const int gi = pgi[q & 1];
-            x.x = ((id.x == gi && fmaf(x.x, s2.x, h2.x) > 0.f) ? s2.x * d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
-            x.y = ((id.y == gi && fmaf(x.y, s2.y, h2.y) > 0.f) ? s2.y * d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
-          }
-          uint32_t w[NSPLIT];
-          split_pair<NSPLIT>(x.x, x.y, w);
 #pragma unroll
-          for (int pl = 0; pl < NSPLIT; ++pl) af[kk][pl][q] = w[pl];
+            for (int i = 0; i < 2; ++i) {
+              float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
+              const int gi = pgi[i];
+              x.x = ((id.x == gi && fmaf(x.x, s2.x, h2.x) > 0.f) ? s2.x * d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
+              x.y = ((id.y == gi && fmaf(x.y, s2.y, h2.y) > 0.f) ? s2.y * d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
+              put(i, x);
+            }
+          } else {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) put(i, *reinterpret_cast<const float2 *>(rt + off(i)));
+          }
         }
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&raw_empty[rs]);    // this warp's rows of the raw stage have been read
+      mma_turn.begin();
       mbar_wait(&b_full[bs], P.b_resident ? 0u : ((it / B_STAGES) & 1u));
       unsigned char *bt = b_ring + (size_t)bs * B_STAGE;
       acc_fence(acc);
@@ -292,6 +339,7 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
                                                       (kb | p | kk) != 0);
       }
       wgmma_commit();
+      mma_turn.end();
       wgmma_wait<0>();     // the A fragments are overwritten by the next k-block
       acc_fence(acc);
       if (!P.b_resident && (threadIdx.x & 127) == 0) mbar_arrive(&b_empty[bs]);
@@ -302,13 +350,15 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
     for (int c = 0; c < BN / 8; ++c) {
       const int col = n0 + c * 8 + 2 * t4;
       float cs0 = 0.f, cs1 = 0.f, cq0 = 0.f, cq1 = 0.f;
+      const float bias0 = P.bias && col < n ? __ldg(P.bias + col) : 0.f;
+      const float bias1 = P.bias && col + 1 < n ? __ldg(P.bias + col + 1) : 0.f;
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         const int row = m0 + rloc[i];
         float v0 = acc[c * 4 + i * 2], v1 = acc[c * 4 + i * 2 + 1];
         if (P.bias) {
-          if (col < n) v0 += __ldg(P.bias + col);
-          if (col + 1 < n) v1 += __ldg(P.bias + col + 1);
+          if (col < n) v0 += bias0;
+          if (col + 1 < n) v1 += bias1;
         }
         if (P.act == 1) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
         if (row < m) {      // rows past m are padding: not stored, excluded from the statistics
@@ -338,6 +388,7 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
       }
     }
   }
+  mma_turn.finish();
   if (P.stats) {
     // fixed-order sum of the eight consumer warps' slices -> this CTA's partial row
     bar_sync(1, 256);

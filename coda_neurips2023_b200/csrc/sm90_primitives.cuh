@@ -160,6 +160,10 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 __device__ __forceinline__ void bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
+// arrive on a named barrier without waiting (the other `threads - arrivals` wait on it with bar_sync)
+__device__ __forceinline__ void bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
 // --------------------------------------------------------------------- descriptors
 // K-major operand tile in shared memory, 128-byte swizzle: rows of 64 16-bit elements (128 B) stored densely,
