@@ -23,6 +23,8 @@
 #include "../../include/coda_gemm.h"
 #include "sm90_primitives.cuh"
 
+#include <type_traits>
+
 using namespace coda;
 
 namespace {
@@ -219,7 +221,6 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
   const int wg = warp >> 2, wl = warp & 3;
   const int g = lane >> 2, t4 = lane & 3;
   const int rloc[2] = {wg * 64 + wl * 16 + g, wg * 64 + wl * 16 + g + 8};   // this thread's two rows of the tile
-  float *my_stats = P.stats ? s_stats + (size_t)warp * 2 * n : nullptr;
   float acc[BN / 2];
   uint32_t it = 0;
   int m0, n0;
@@ -229,13 +230,6 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
   // same time, with the pipe idle.
   Alternation mma_turn{wg, false};
   for (long long t = 0; tile_at(t, m0, n0); ++t) {
-    // pooled mode: the 16 rows of a warp lie in one group (group % 32 == 0); index of each row within it
-    int pgt = 0, pgi[2] = {0, 0};
-    if (pooled) {
-      pgt = P.group >= BM ? 0 : rloc[0] / P.group;
-#pragma unroll
-      for (int i = 0; i < 2; ++i) pgi[i] = (int)(((long long)m0 + rloc[i]) % P.group);
-    }
     for (int kb = 0; kb < nkb; ++kb, ++it) {
       const int rs = it % nraw, bs = P.b_resident ? kb : (int)(it % B_STAGES);
       mbar_wait(&raw_full[rs], (it / nraw) & 1u);
@@ -244,82 +238,103 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
       // A fragments of the four 16-deep k-steps: register q of step kk holds (row rloc[q & 1], columns
       // 16 kk + 8 (q >> 1) + 2 t4 + {0, 1})
       uint32_t af[BK / 16][NSPLIT][4];
+      // The prologue's mode is the same for the whole launch.  The plain and BN+ReLU prologues are branched on once
+      // per k-block (MODE >= 0): their eight column pairs are then straight-line code, whose shared-memory and
+      // per-column loads are issued ahead of the arithmetic instead of as one dependent chain per column pair.  The
+      // BatchNorm-backward prologues (MODE < 0) keep one branch per column pair: hoisting their two inputs and up to
+      // four per-column vectors would not fit in the registers.
+      auto convert = [&](auto mode_tag) {
+        constexpr int MODE = decltype(mode_tag)::value;
+        const int mode = MODE >= 0 ? MODE : P.mode;
+        // pooled mode: the 16 rows of a warp lie in one group (group % 32 == 0); index of each row within it
+        int pgt = 0, pgi[2] = {0, 0};
+        if (MODE < 0 && pooled) {
+          pgt = P.group >= BM ? 0 : rloc[0] / P.group;
 #pragma unroll
-      for (int kk = 0; kk < BK / 16; ++kk) {
+          for (int i = 0; i < 2; ++i) pgi[i] = (int)(((long long)m0 + rloc[i]) % P.group);
+        }
 #pragma unroll
-        for (int c2 = 0; c2 < 2; ++c2) {
-          // registers q = 2 c2 + i, i = 0, 1 (rows rloc[i]) share their columns and so the per-column operands of the
-          // prologue: those are read once for both rows
-          const int col = kk * 16 + c2 * 8 + 2 * t4;   // column of the k-block (even)
-          const int kc = k0 + col;
-          auto off = [&](int i) {
-            const int row = rloc[i];
-            return (uint32_t)(col >> 5) * (RAW_TILE / 2) + (uint32_t)row * 128u +
-                   ((uint32_t)(((col & 31) >> 2) ^ (row & 7)) << 4) + (uint32_t)(col & 3) * 4u;
-          };
-          auto put = [&](int i, float2 x) {
-            uint32_t w[NSPLIT];
-            split_pair<NSPLIT>(x.x, x.y, w);
+        for (int kk = 0; kk < BK / 16; ++kk) {
 #pragma unroll
-            for (int pl = 0; pl < NSPLIT; ++pl) af[kk][pl][c2 * 2 + i] = w[pl];
-          };
-          auto ld2 = [&](const float *v) { return __ldg(reinterpret_cast<const float2 *>(v + kc)); };
-          if (P.mode == CODA_A32_AFFINE_RELU) {
-            const float2 s2 = ld2(P.scale), h2 = ld2(P.shift);
+          for (int c2 = 0; c2 < 2; ++c2) {
+            // registers q = 2 c2 + i, i = 0, 1 (rows rloc[i]) share their columns and so the per-column operands of the
+            // prologue: those are read once for both rows
+            const int col = kk * 16 + c2 * 8 + 2 * t4;   // column of the k-block (even)
+            const int kc = k0 + col;
+            auto off = [&](int i) {
+              const int row = rloc[i];
+              return (uint32_t)(col >> 5) * (RAW_TILE / 2) + (uint32_t)row * 128u +
+                     ((uint32_t)(((col & 31) >> 2) ^ (row & 7)) << 4) + (uint32_t)(col & 3) * 4u;
+            };
+            auto put = [&](int i, float2 x) {
+              uint32_t w[NSPLIT];
+              split_pair<NSPLIT>(x.x, x.y, w);
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
-              x.x = fmaxf(fmaf(x.x, s2.x, h2.x), 0.f);
-              x.y = fmaxf(fmaf(x.y, s2.y, h2.y), 0.f);
-              put(i, x);
+              for (int pl = 0; pl < NSPLIT; ++pl) af[kk][pl][c2 * 2 + i] = w[pl];
+            };
+            auto ld2 = [&](const float *v) { return __ldg(reinterpret_cast<const float2 *>(v + kc)); };
+            if (mode == CODA_A32_AFFINE_RELU) {
+              const float2 s2 = ld2(P.scale), h2 = ld2(P.shift);
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
+                x.x = fmaxf(fmaf(x.x, s2.x, h2.x), 0.f);
+                x.y = fmaxf(fmaf(x.y, s2.y, h2.y), 0.f);
+                put(i, x);
+              }
+            } else if (mode == CODA_A32_BN_BWD) {
+              // x = y (pre-BN activation), d = gradient of relu(bn(y)).  With s = gamma * invstd, t = beta_bn - mean * s:
+              //   dy = s * ([s y + t > 0] d - s1/N - xhat s2/N) = [s y + t > 0] * s * d + alpha * y + beta
+              //   alpha = -s * invstd * s2 / N,  beta = -s * s1 / N - alpha * mean        (host: coda_bn_bwd_coefs)
+              const float2 s2 = ld2(P.scale), h2 = ld2(P.shift), a2 = ld2(P.alpha), b2 = ld2(P.beta);
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
+                const float2 d = *reinterpret_cast<const float2 *>(rt + RAW_TILE + off(i));
+                x.x = (fmaf(x.x, s2.x, h2.x) > 0.f ? s2.x * d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
+                x.y = (fmaf(x.y, s2.y, h2.y) > 0.f ? s2.y * d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
+                put(i, x);
+              }
+            } else if (mode == CODA_A32_BN_BWD_POOLED_PRE) {
+              // pre-masked, pre-scaled pooled gradient: one compare + select + FMA + add per element
+              const unsigned char *px = rt + RAW_TILE + pgt * 320;
+              const float2 a2 = ld2(P.alpha), b2 = ld2(P.beta);
+              const float2 d = *reinterpret_cast<const float2 *>(px + col * 4);
+              const uchar2 id = *reinterpret_cast<const uchar2 *>(px + 256 + col);
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
+                const int gi = pgi[i];
+                x.x = (id.x == gi ? d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
+                x.y = (id.y == gi ? d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
+                put(i, x);
+              }
+            } else if (mode == CODA_A32_BN_BWD_POOLED) {
+              // the layer output was max-pooled over `group` rows: only the arg-max row of a (group, channel)
+              // carries the incoming gradient dpooled[g][c]
+              const unsigned char *px = rt + RAW_TILE + pgt * 320;     // staged by the producer with the raw tile
+              const float2 s2 = ld2(P.scale), h2 = ld2(P.shift), a2 = ld2(P.alpha), b2 = ld2(P.beta);
+              const float2 d = *reinterpret_cast<const float2 *>(px + col * 4);
+              const uchar2 id = *reinterpret_cast<const uchar2 *>(px + 256 + col);
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
+                const int gi = pgi[i];
+                x.x = ((id.x == gi && fmaf(x.x, s2.x, h2.x) > 0.f) ? s2.x * d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
+                x.y = ((id.y == gi && fmaf(x.y, s2.y, h2.y) > 0.f) ? s2.y * d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
+                put(i, x);
+              }
+            } else {
+#pragma unroll
+              for (int i = 0; i < 2; ++i) put(i, *reinterpret_cast<const float2 *>(rt + off(i)));
             }
-          } else if (P.mode == CODA_A32_BN_BWD) {
-            // x = y (pre-BN activation), d = gradient of relu(bn(y)).  With s = gamma * invstd, t = beta_bn - mean * s:
-            //   dy = s * ([s y + t > 0] d - s1/N - xhat s2/N) = [s y + t > 0] * s * d + alpha * y + beta
-            //   alpha = -s * invstd * s2 / N,  beta = -s * s1 / N - alpha * mean        (host: coda_bn_bwd_coefs)
-            const float2 s2 = ld2(P.scale), h2 = ld2(P.shift), a2 = ld2(P.alpha), b2 = ld2(P.beta);
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
-              const float2 d = *reinterpret_cast<const float2 *>(rt + RAW_TILE + off(i));
-              x.x = (fmaf(x.x, s2.x, h2.x) > 0.f ? s2.x * d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
-              x.y = (fmaf(x.y, s2.y, h2.y) > 0.f ? s2.y * d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
-              put(i, x);
-            }
-          } else if (P.mode == CODA_A32_BN_BWD_POOLED_PRE) {
-            // pre-masked, pre-scaled pooled gradient: one compare + select + FMA + add per element
-            const unsigned char *px = rt + RAW_TILE + pgt * 320;
-            const float2 a2 = ld2(P.alpha), b2 = ld2(P.beta);
-            const float2 d = *reinterpret_cast<const float2 *>(px + col * 4);
-            const uchar2 id = *reinterpret_cast<const uchar2 *>(px + 256 + col);
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
-              const int gi = pgi[i];
-              x.x = (id.x == gi ? d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
-              x.y = (id.y == gi ? d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
-              put(i, x);
-            }
-          } else if (P.mode == CODA_A32_BN_BWD_POOLED) {
-            // the layer output was max-pooled over `group` rows: only the arg-max row of a (group, channel)
-            // carries the incoming gradient dpooled[g][c]
-            const unsigned char *px = rt + RAW_TILE + pgt * 320;     // staged by the producer with the raw tile
-            const float2 s2 = ld2(P.scale), h2 = ld2(P.shift), a2 = ld2(P.alpha), b2 = ld2(P.beta);
-            const float2 d = *reinterpret_cast<const float2 *>(px + col * 4);
-            const uchar2 id = *reinterpret_cast<const uchar2 *>(px + 256 + col);
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
-              const int gi = pgi[i];
-              x.x = ((id.x == gi && fmaf(x.x, s2.x, h2.x) > 0.f) ? s2.x * d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
-              x.y = ((id.y == gi && fmaf(x.y, s2.y, h2.y) > 0.f) ? s2.y * d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
-              put(i, x);
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 2; ++i) put(i, *reinterpret_cast<const float2 *>(rt + off(i)));
           }
         }
+      };
+      switch (P.mode) {
+        case CODA_A32_PLAIN: convert(std::integral_constant<int, CODA_A32_PLAIN>{}); break;
+        case CODA_A32_AFFINE_RELU: convert(std::integral_constant<int, CODA_A32_AFFINE_RELU>{}); break;
+        default: convert(std::integral_constant<int, -1>{}); break;
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&raw_empty[rs]);    // this warp's rows of the raw stage have been read
@@ -346,44 +361,65 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
     }
 
     // ===== epilogue: registers -> (+bias, ReLU) -> global, optional column statistics =====
+    // Per chunk of EPI_C column groups, three passes (stores and per-thread sums, the shuffle tree, the shared-memory
+    // update) rather than one column group at a time, so that the groups' shuffle and shared-memory latencies
+    // overlap.  Each sum is formed in the same order as group by group.
+    constexpr int EPI_C = 4;
 #pragma unroll
-    for (int c = 0; c < BN / 8; ++c) {
-      const int col = n0 + c * 8 + 2 * t4;
-      float cs0 = 0.f, cs1 = 0.f, cq0 = 0.f, cq1 = 0.f;
-      const float bias0 = P.bias && col < n ? __ldg(P.bias + col) : 0.f;
-      const float bias1 = P.bias && col + 1 < n ? __ldg(P.bias + col + 1) : 0.f;
+    for (int cb = 0; cb < BN / 8; cb += EPI_C) {
+      float csum[EPI_C][2], csq[EPI_C][2];
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int row = m0 + rloc[i];
-        float v0 = acc[c * 4 + i * 2], v1 = acc[c * 4 + i * 2 + 1];
-        if (P.bias) {
-          if (col < n) v0 += bias0;
-          if (col + 1 < n) v1 += bias1;
-        }
-        if (P.act == 1) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-        if (row < m) {      // rows past m are padding: not stored, excluded from the statistics
-          float *crow = P.c + (size_t)row * P.ldc;
-          if (col + 1 < n) {
-            *reinterpret_cast<float2 *>(crow + col) = make_float2(v0, v1);   // ldc % 4 == 0, col even
-          } else if (col < n) {
-            crow[col] = v0;
+      for (int ci = 0; ci < EPI_C; ++ci) {
+        const int c = cb + ci;
+        const int col = n0 + c * 8 + 2 * t4;
+        float cs0 = 0.f, cs1 = 0.f, cq0 = 0.f, cq1 = 0.f;
+        const float bias0 = P.bias && col < n ? __ldg(P.bias + col) : 0.f;
+        const float bias1 = P.bias && col + 1 < n ? __ldg(P.bias + col + 1) : 0.f;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int row = m0 + rloc[i];
+          float v0 = acc[c * 4 + i * 2], v1 = acc[c * 4 + i * 2 + 1];
+          if (P.bias) {
+            if (col < n) v0 += bias0;
+            if (col + 1 < n) v1 += bias1;
           }
-          cs0 += v0; cq0 = fmaf(v0, v0, cq0);
-          cs1 += v1; cq1 = fmaf(v1, v1, cq1);
+          if (P.act == 1) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+          if (row < m) {      // rows past m are padding: not stored, excluded from the statistics
+            float *crow = P.c + (size_t)row * P.ldc;
+            if (col + 1 < n) {
+              *reinterpret_cast<float2 *>(crow + col) = make_float2(v0, v1);   // ldc % 4 == 0, col even
+            } else if (col < n) {
+              crow[col] = v0;
+            }
+            cs0 += v0; cq0 = fmaf(v0, v0, cq0);
+            cs1 += v1; cq1 = fmaf(v1, v1, cq1);
+          }
         }
+        csum[ci][0] = cs0; csum[ci][1] = cs1; csq[ci][0] = cq0; csq[ci][1] = cq1;
       }
-      if (my_stats) {
+      if (P.stats) {
+        float *my_stats = s_stats + warp * 2 * n;   // this warp's [2][n] slice
         // column sums over the warp's 16 rows: reduce across the eight row groups (lane bits 2..4)
 #pragma unroll
         for (int o = 4; o < 32; o <<= 1) {
-          cs0 += __shfl_xor_sync(0xffffffffu, cs0, o);
-          cs1 += __shfl_xor_sync(0xffffffffu, cs1, o);
-          cq0 += __shfl_xor_sync(0xffffffffu, cq0, o);
-          cq1 += __shfl_xor_sync(0xffffffffu, cq1, o);
+#pragma unroll
+          for (int ci = 0; ci < EPI_C; ++ci) {
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+              csum[ci][j] += __shfl_xor_sync(0xffffffffu, csum[ci][j], o);
+              csq[ci][j] += __shfl_xor_sync(0xffffffffu, csq[ci][j], o);
+            }
+          }
         }
         if (g == 0) {
-          if (col < n) { my_stats[col] += cs0; my_stats[n + col] += cq0; }
-          if (col + 1 < n) { my_stats[col + 1] += cs1; my_stats[n + col + 1] += cq1; }
+#pragma unroll
+          for (int ci = 0; ci < EPI_C; ++ci) {
+            const int col = n0 + (cb + ci) * 8 + 2 * t4;
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+              if (col + j < n) { my_stats[col + j] += csum[ci][j]; my_stats[n + col + j] += csq[ci][j]; }
+            }
+          }
         }
       }
     }

@@ -1,5 +1,6 @@
 """Micro-benchmark of the fp32-A wgmma GEMMs (CUDA events, kernel alone, warm) on the step's shapes.
-Prints one JSON line per case: ms, useful TFLOP/s, algorithmic GB/s."""
+Prints one JSON line per case: ms, useful TFLOP/s, algorithmic GB/s, and for the 1M-row launches the HBM bound
+(algorithmic bytes at 3.35 TB/s) and the fraction of it reached."""
 import json
 import sys
 from pathlib import Path
@@ -8,6 +9,8 @@ import torch
 
 sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 from coda_neurips2023_b200 import ops  # noqa: E402
+
+HBM_BPS = 3.35e12
 
 
 def timeit(fn, reps=20, warm=3):
@@ -54,9 +57,14 @@ def main():
         ms = timeit(fn)
         flops = 2.0 * m * n * k
         nbytes = 4.0 * m * k + 4.0 * m * n + 2.0 * ns * n * k
-        print(json.dumps({"case": name, "ms": round(ms, 4), "useful_tflops": round(flops / ms / 1e9, 1),
-                          "tensor_pipe_tflops": round(flops * {2: 3, 3: 6}[ns] / ms / 1e9, 1),
-                          "algorithmic_GBps": round(nbytes / ms / 1e6, 1)}))
+        rec = {"case": name, "ms": round(ms, 4), "useful_tflops": round(flops / ms / 1e9, 1),
+               "tensor_pipe_tflops": round(flops * {2: 3, 3: 6}[ns] / ms / 1e9, 1),
+               "algorithmic_GBps": round(nbytes / ms / 1e6, 1)}
+        if m >= 1 << 20:
+            # the 1M-row launches are bounded by HBM: algorithmic bytes at the H100 SXM data-sheet 3.35 TB/s
+            rec["hbm_bound_ms"] = round(nbytes / HBM_BPS * 1e3, 4)
+            rec["hbm_bound_frac"] = round(nbytes / HBM_BPS * 1e3 / ms, 3)
+        print(json.dumps(rec))
     # weight gradient from fp32 rows
     for name, rows, m, n in [("dW 16384 rows 512x512", 16384, 512, 512), ("SA dW2 1M rows 256x128", 1 << 20, 256, 128),
                              ("SA dW1 1M rows 128x64", 1 << 20, 128, 64)]:
