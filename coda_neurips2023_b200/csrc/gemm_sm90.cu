@@ -308,6 +308,146 @@ gemm_nt_kernel(const __grid_constant__ GemmMaps maps, int m, int n, int kpad, in
   }
 }
 
+// ------------------------------------------------------------------ fp16 ping-pong GEMM (the CLIP tower's shapes)
+// C = epilogue(A B^T) with one fp16 plane per operand, batch 1, fp16 output, n % BN == 0.  384 threads:
+//   warpgroup 2    : TMA producer (setmaxnreg 40; one elected lane of its first warp issues the copies)
+//   warpgroups 0, 1: consumers (setmaxnreg 232).  Warpgroup c owns whole 128 x BN tiles: the CTA's tiles
+//                    j = c, c + 2, ... of its persistent work list, rows [0, 64) and [64, 128) in two accumulators.
+// ptxas allocates the whole kernel within the 168 registers of the launch bound: BN = 128 (128 accumulator registers)
+// fits with no spills, BN = 192 spills.
+// The producer fills one stage ring in tile order; each stage is consumed (and released) by the owner of its tile.
+// The two consumers issue their main loops in turn: warpgroup c starts tile j once warpgroup c ^ 1 has issued the last
+// wgmma of tile j - 1 (named barrier 1 + c).  So one warpgroup's epilogue runs while the other's wgmmas keep the tensor
+// pipe busy.  Every element sums its k-blocks and k16 steps in the same order as gemm_nt_kernel, then takes the same
+// epilogue and one fp16 rounding: C has the same bits.
+constexpr int PP_THREADS = 384;
+constexpr int PP_PRODUCER_REGS = 40, PP_MMA_REGS = 232;   // 128 x 40 + 256 x 232 <= 64 K registers
+enum PpEpilogue { PP_NONE = 0, PP_BIAS = 1, PP_BIAS_GELU = 2, PP_BIAS_RES = 3 };
+
+template <int BN, int STAGES, int EPI>
+__global__ void __launch_bounds__(PP_THREADS, 1)
+gemm_f16_pp_kernel(const __grid_constant__ GemmMaps maps, int m, int n, int nkb, const float *__restrict__ bias,
+                   const __half *__restrict__ residual, long long ldr, __half *__restrict__ c, long long ldc) {
+  constexpr int A_TILE = BM * BK * 2;
+  constexpr int STAGE = A_TILE + BN * BK * 2;
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  __shared__ __align__(8) uint64_t full_bar[STAGES];
+  __shared__ __align__(8) uint64_t empty_bar[STAGES];
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tiles_m = (m + BM - 1) / BM, tiles_n = n / BN;
+  const int ntiles = tiles_m * tiles_n;
+  const bool n_fast = tiles_n <= tiles_m;   // the tile order of gemm_nt_kernel
+  auto decode = [&](int w, int &m0, int &n0) {
+    const int tm = n_fast ? w / tiles_n : w % tiles_m, tn = n_fast ? w % tiles_n : w / tiles_m;
+    m0 = tm * BM; n0 = tn * BN;
+  };
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
+    mbar_fence_init_cluster();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // ===== TMA producer warpgroup =====
+    setmaxnreg_dec<PP_PRODUCER_REGS>();
+    if (warp != 8) return;
+    if (lane == 0) { prefetch_tmap(&maps.a[0]); prefetch_tmap(&maps.b[0]); }
+    uint32_t it = 0;
+    for (int w = blockIdx.x; w < ntiles; w += gridDim.x) {
+      int m0, n0;
+      decode(w, m0, n0);
+      for (int kb = 0; kb < nkb; ++kb, ++it) {
+        const int s = it % STAGES;
+        mbar_wait(&empty_bar[s], ((it / STAGES) & 1u) ^ 1u);
+        if (elect_one_sync()) {
+          mbar_arrive_expect_tx(&full_bar[s], (uint32_t)STAGE);
+          unsigned char *st = smem + (size_t)s * STAGE;
+          tma_load_3d(st, &maps.a[0], &full_bar[s], kb * BK, m0, 0);
+          tma_load_3d(st + A_TILE, &maps.b[0], &full_bar[s], kb * BK, n0, 0);
+        }
+        __syncwarp();
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<PP_MMA_REGS>();
+
+  // ===== consumers: warpgroup wg owns every other tile of the CTA; accumulators for rows [0, 64) and [64, 128) =====
+  const int wg = warp >> 2, wl = warp & 3;
+  const int g = lane >> 2, t = lane & 3;
+  float acc[2][BN / 2];
+  // ring position of the tile's first k-block: the CTA's j-th tile starts at j * nkb
+  uint32_t it = (uint32_t)(wg * nkb);
+  for (int w = blockIdx.x + wg * gridDim.x; w < ntiles; w += 2 * gridDim.x, it += 2 * nkb) {
+    int m0, n0;
+    decode(w, m0, n0);
+    const bool other_next = w + (int)gridDim.x < ntiles;   // the other warpgroup has the CTA's next tile
+    // wait for the turn: the other warpgroup has issued all wgmmas of the CTA's previous tile
+    if (wg == 1 || w != (int)blockIdx.x) bar_sync(1 + wg, 256);
+    for (int kb = 0; kb < nkb; ++kb) {
+      const uint32_t i = it + kb;
+      const int s = i % STAGES;
+      mbar_wait(&full_bar[s], (i / STAGES) & 1u);
+      unsigned char *st = smem + (size_t)s * STAGE;
+      acc_fence(acc[0]);
+      acc_fence(acc[1]);
+      wgmma_fence();
+      const uint64_t ad = gmma_desc_k_sw128(st), bd = gmma_desc_k_sw128(st + A_TILE);
+#pragma unroll
+      for (int kk = 0; kk < BK / 16; ++kk) {
+        const uint64_t b = gmma_desc_advance(bd, kk * 32);
+        Wgmma<BN, true>::template ss<0, 0>(acc[0], gmma_desc_advance(ad, kk * 32), b, (kb | kk) != 0);
+        Wgmma<BN, true>::template ss<0, 0>(acc[1], gmma_desc_advance(ad, 8192 + kk * 32), b, (kb | kk) != 0);
+      }
+      wgmma_commit();
+      if (kb == nkb - 1 && other_next) bar_arrive(1 + (wg ^ 1), 256);   // hand the turn over
+      // the previous k-block's MMAs are complete: release its stage
+      wgmma_wait<1>();
+      acc_fence(acc[0]);
+      acc_fence(acc[1]);
+      if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
+    }
+
+    // bias of the thread's column pairs, read once per tile while the last k-block's MMAs run
+    float2 bv[BN / 8];
+    if (EPI != PP_NONE) {
+#pragma unroll
+      for (int cc = 0; cc < BN / 8; ++cc) bv[cc] = __ldg(reinterpret_cast<const float2 *>(bias + n0 + cc * 8 + 2 * t));
+    }
+    wgmma_wait<0>();
+    acc_fence(acc[0]);
+    acc_fence(acc[1]);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[(it + nkb - 1) % STAGES]);
+
+    // ===== epilogue: fp32 accumulator + bias, activation, + residual, one fp16 rounding =====
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int row = m0 + h * 64 + wl * 16 + g + 8 * r;
+        if (row >= m) continue;
+        __half *crow = c + (size_t)row * ldc + n0 + 2 * t;
+        const __half *rrow = EPI == PP_BIAS_RES ? residual + (size_t)row * ldr + n0 + 2 * t : nullptr;
+#pragma unroll
+        for (int cc = 0; cc < BN / 8; ++cc) {
+          float v0 = acc[h][cc * 4 + r * 2], v1 = acc[h][cc * 4 + r * 2 + 1];
+          if (EPI != PP_NONE) { v0 += bv[cc].x; v1 += bv[cc].y; }
+          if (EPI == PP_BIAS_GELU) { v0 = apply_act(v0, 2); v1 = apply_act(v1, 2); }
+          if (EPI == PP_BIAS_RES) {
+            const __half2 rv = *reinterpret_cast<const __half2 *>(rrow + cc * 8);
+            v0 += __low2float(rv);
+            v1 += __high2float(rv);
+          }
+          *reinterpret_cast<__half2 *>(crow + cc * 8) = __floats2half2_rn(v0, v1);
+        }
+      }
+    }
+  }
+}
+
 int device_sms() {
   static int num_sms = 0;
   if (!num_sms) {
@@ -363,6 +503,25 @@ int launch_gemm(const GemmMaps &maps, int batch, int m, int n, int kpad, int b_b
     splitk_reduce_kernel<<<(unsigned)(blocks < 8 * sms ? blocks : 8 * sms), 256, 0, s>>>(partial, ksplit, m, n, batch, BM,
                                                                                           BN, bias, c, ldc, c_batch_stride);
   }
+  return launch_status();
+}
+
+template <int BN, int STAGES, int EPI>
+int launch_gemm_f16_pp(const GemmMaps &maps, int m, int n, int kpad, const float *bias, const void *residual,
+                       long long ldr, void *c, long long ldc, cudaStream_t s) {
+  constexpr size_t smem = (size_t)STAGES * (BM * BK * 2 + BN * BK * 2) + 1024;
+  static_assert(smem <= 227 * 1024, "smem budget");
+  auto kern = gemm_f16_pp_kernel<BN, STAGES, EPI>;
+  static bool configured = false;  // once per template instance
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return (int)e;
+    configured = true;
+  }
+  const int sms = device_sms();
+  const int tiles = (m + BM - 1) / BM * (n / BN);
+  kern<<<(unsigned)(tiles < sms ? tiles : sms), PP_THREADS, smem, s>>>(
+      maps, m, n, kpad / BK, bias, reinterpret_cast<const __half *>(residual), ldr, reinterpret_cast<__half *>(c), ldc);
   return launch_status();
 }
 
@@ -436,7 +595,20 @@ int coda_gemm_nt_res(int nsplit, int is_fp16, int batch, int m, int n, int kpad,
   // fp16 tower GEMMs with wide outputs: a 128 x 256 tile moves 48 KB per k-block for twice the flops of a 128 x 128
   // tile (32 KB).  N = 768 (attention / MLP output projections of the ViT) takes 192-wide tiles: more flops per
   // byte than 128-wide ones, and a 768-wide row is still an exact number of tiles.
-  const int bn = n <= 64 ? 64
+  // The ping-pong kernel takes fp16-output calls with the epilogues the CLIP tower uses, 128-wide tiles that divide n,
+  // 16-byte aligned outputs / residual rows, and at least two tiles per SM: with fewer, one warpgroup per SM would sit
+  // idle and the 288-thread kernel, whose warpgroups share each tile, is the better fit.
+  constexpr int PP_BN = 128;
+  const int pp_epi = !bias ? (relu == 0 && !residual ? PP_NONE : -1)
+                     : relu == 0 ? (residual ? PP_BIAS_RES : PP_BIAS)
+                     : (relu == 2 && !residual) ? PP_BIAS_GELU : -1;
+  const long long pp_tiles = (long long)((m + BM - 1) / BM) * (n / PP_BN);   // int tile indices in the kernel
+  const bool pp = is_fp16 && out_half && batch == 1 && pp_epi >= 0 && n % PP_BN == 0 &&
+                  pp_tiles >= 2LL * device_sms() && pp_tiles <= INT_MAX && ldc % 8 == 0 &&
+                  ((uintptr_t)c & 15) == 0 && ((uintptr_t)bias & 7) == 0 &&
+                  (!residual || (ldr % 8 == 0 && ((uintptr_t)residual & 15) == 0));
+  const int bn = pp ? PP_BN
+                 : n <= 64 ? 64
                  : (is_fp16 && n % 256 == 0 && n >= 1536) ? 256
                  : (is_fp16 && n % 192 == 0 && n >= 384)  ? 192
                                                           : 128;
@@ -455,6 +627,15 @@ int coda_gemm_nt_res(int nsplit, int is_fp16, int batch, int m, int n, int kpad,
 #define CODA_GEMM(NS, BN_, ST, F16) \
   return launch_gemm<NS, BN_, ST, F16>(maps, batch, m, n, kpad, bb, bias, relu, c, ldc, c_batch_stride, s, out_half, \
                                        residual, ldr)
+  if (pp) {
+#define CODA_GEMM_PP(EPI) \
+  return launch_gemm_f16_pp<PP_BN, 6, EPI>(maps, m, n, kpad, bias, residual, ldr, c, ldc, s)
+    if (pp_epi == PP_NONE) CODA_GEMM_PP(PP_NONE);
+    if (pp_epi == PP_BIAS) CODA_GEMM_PP(PP_BIAS);
+    if (pp_epi == PP_BIAS_GELU) CODA_GEMM_PP(PP_BIAS_GELU);
+    CODA_GEMM_PP(PP_BIAS_RES);
+#undef CODA_GEMM_PP
+  }
   if (is_fp16) {
     if (bn == 64) CODA_GEMM(1, 64, 6, true);
     if (bn == 256) CODA_GEMM(1, 256, 4, true);
