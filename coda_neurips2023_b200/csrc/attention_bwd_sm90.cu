@@ -37,7 +37,7 @@ using namespace coda::attn;
 namespace {
 
 constexpr int NS = 2;           // planes per operand in the backward
-constexpr int NPROD = 3;
+constexpr int NPROD = n_products(NS);
 
 // Per-query values of the backward, qv[bh][q] = (lse * log2 e, D = sum_d dO * O) with dO, O (Lq, B, H*hd); rows
 // Lq..Lqp-1 (padding to whole 64-query tiles) are zero, so a tile's 64 entries are one aligned 512-byte block.
@@ -108,7 +108,7 @@ __device__ __forceinline__ void scores2_issue(float (&s)[32], float (&t)[32], co
   for (int p = 0; p < NPROD; ++p)
 #pragma unroll
     for (int kb = 0; kb < KB; ++kb) {
-      const int xo = a_pa(NS, p) * res_plane + kb * 8192, yo = a_pb(NS, p) * tile_plane + kb * 8192;
+      const int xo = prod_a(NS, p) * res_plane + kb * 8192, yo = prod_b(NS, p) * tile_plane + kb * 8192;
       const uint64_t ax = gmma_desc_k_sw128(x0 + xo), by = gmma_desc_k_sw128(y0 + yo);
       const uint64_t ax1 = gmma_desc_k_sw128(x1 + xo), by1 = gmma_desc_k_sw128(y1 + yo);
 #pragma unroll
@@ -133,7 +133,7 @@ attn_bwd_dq_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B, 
   constexpr int KB = C::KB, NST = C::NST;
   if (seed_dev) seed += __ldg(seed_dev);
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  unsigned char *smem = smem_align1024(smem_raw);
   __shared__ __align__(8) uint64_t q_full, kv_full[NST], kv_empty[NST];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 64 * NWG, bh = blockIdx.y;
@@ -242,10 +242,10 @@ attn_bwd_dq_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B, 
     wgmma_fence();
 #pragma unroll
     for (int p = 0; p < NPROD; ++p) {
-      const uint64_t bk = gmma_desc_mn_sw128(ks + a_pb(NS, p) * C::TILE_PLANE);
+      const uint64_t bk = gmma_desc_mn_sw128(ks + prod_b(NS, p) * C::TILE_PLANE);
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk)   // 16 keys: 16 rows x 128 B of K_j
-        Wgmma<HD, false>::template rs<1>(dq_acc, af[kk][a_pa(NS, p)], gmma_desc_advance(bk, kk * 16 * 128), 1);
+        Wgmma<HD, false>::template rs<1>(dq_acc, af[kk][prod_a(NS, p)], gmma_desc_advance(bk, kk * 16 * 128), 1);
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -276,7 +276,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B,
   constexpr int KB = C::KB, NST = C::NST;
   if (seed_dev) seed += __ldg(seed_dev);
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  unsigned char *smem = smem_align1024(smem_raw);
   __shared__ __align__(8) uint64_t kv_full, q_full[NST], q_empty[NST];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int k0 = blockIdx.x * 64 * NWG, bh = blockIdx.y;
@@ -401,12 +401,12 @@ attn_bwd_dkv_kernel(const __grid_constant__ BwdMaps maps, int Lq, int Lk, int B,
     wgmma_fence();
 #pragma unroll
     for (int p = 0; p < NPROD; ++p) {
-      const uint64_t bo = gmma_desc_mn_sw128(dos + a_pb(NS, p) * C::TILE_PLANE);
-      const uint64_t bq = gmma_desc_mn_sw128(qs + a_pb(NS, p) * C::TILE_PLANE);
+      const uint64_t bo = gmma_desc_mn_sw128(dos + prod_b(NS, p) * C::TILE_PLANE);
+      const uint64_t bq = gmma_desc_mn_sw128(qs + prod_b(NS, p) * C::TILE_PLANE);
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {  // 16 queries: 16 rows x 128 B of dO_i / Qs_i
-        Wgmma<HD, false>::template rs<1>(dv_acc, pf[kk][a_pa(NS, p)], gmma_desc_advance(bo, kk * 16 * 128), 1);
-        Wgmma<HD, false>::template rs<1>(dk_acc, sf[kk][a_pa(NS, p)], gmma_desc_advance(bq, kk * 16 * 128), 1);
+        Wgmma<HD, false>::template rs<1>(dv_acc, pf[kk][prod_a(NS, p)], gmma_desc_advance(bo, kk * 16 * 128), 1);
+        Wgmma<HD, false>::template rs<1>(dk_acc, sf[kk][prod_a(NS, p)], gmma_desc_advance(bq, kk * 16 * 128), 1);
       }
     }
     wgmma_commit();
@@ -436,15 +436,8 @@ int launch_bwd(const BwdMaps &mq, const BwdMaps &mk, int b, int h, int lq, int l
                const unsigned int *seed_dev, cudaStream_t s) {
   constexpr int NWG = HD == 64 ? 2 : 1;
   using C = BwdCfg<HD, NWG>;
-  static bool configured = false;  // once per template instance
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(attn_bwd_dq_kernel<HD, NWG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         C::TOTAL + 1024);
-    if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(attn_bwd_dkv_kernel<HD, NWG>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::TOTAL + 1024);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
+  if (const int st = raise_smem_limit<attn_bwd_dq_kernel<HD, NWG>>(C::TOTAL + 1024)) return st;
+  if (const int st = raise_smem_limit<attn_bwd_dkv_kernel<HD, NWG>>(C::TOTAL + 1024)) return st;
   const int bh = b * h, rows = 64 * NWG;
   attn_bwd_dq_kernel<HD, NWG><<<dim3((lq + rows - 1) / rows, bh), C::THREADS, C::TOTAL + 1024, s>>>(
       mq, lq, lk, b, h, scale, qv, dq, ld_dq, mask_q, dropout_p, seed, seed_dev);

@@ -1,5 +1,5 @@
 // Shared pieces of the wgmma attention kernels (forward: attention_sm90.cu, backward:
-// attention_bwd_sm90.cu): tile sizes, split-product tables, bf16 plane splitting, dropout hash.
+// attention_bwd_sm90.cu): tile sizes, operand packing, dropout hash.
 #pragma once
 #include <math.h>
 
@@ -13,29 +13,7 @@ constexpr int KT = 64;    // keys per tile (one 128-byte swizzle span of bf16)
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr float LN2 = 0.6931471805599453f;
 
-__host__ __device__ constexpr int a_nprod(int ns) { return ns == 1 ? 1 : (ns == 2 ? 3 : 6); }
-__host__ __device__ constexpr int a_pa(int ns, int p) {
-  return ns == 1 ? 0 : ns == 2 ? (p == 0 ? 1 : 0) : (p == 0 ? 1 : p == 1 ? 2 : p == 2 ? 0 : p == 3 ? 1 : 0);
-}
-__host__ __device__ constexpr int a_pb(int ns, int p) {
-  return ns == 1 ? 0 : ns == 2 ? (p == 1 ? 1 : 0) : (p == 0 ? 1 : p == 1 ? 0 : p == 2 ? 2 : p == 3 ? 0 : p == 4 ? 1 : 0);
-}
-
 // ------------------------------------------------------------------ operand packing
-// src (L, B, H*HD) fp32 sequence-first.  mode 0: planes [ns][B*H][L][HD]   (q, k; K-major rows)
-//                                        mode 1: planes [ns][B*H][HD][Lpad] (v^T; keys contiguous)
-template <int NSPLIT>
-__device__ __forceinline__ void split3(float x, __nv_bfloat16 *dst, size_t plane_stride) {
-  const __nv_bfloat16 h = __float2bfloat16_rn(x);
-  dst[0] = h;
-  if (NSPLIT >= 2) {
-    const float r1 = x - __bfloat162float(h);
-    const __nv_bfloat16 m = __float2bfloat16_rn(r1);
-    dst[plane_stride] = m;
-    if (NSPLIT >= 3) dst[2 * plane_stride] = __float2bfloat16_rn(r1 - __bfloat162float(m));
-  }
-}
-
 // Several (L, B, H*hd) tensors (fp32 or fp16, row stride `ld` elements: slices of a fused qkv projection are
 // read in place) -> row planes [NS][B*H][L][hd] in ONE launch: blockIdx.y selects the tensor, a thread converts
 // four consecutive head-dim elements (one 16- or 8-byte load, one 8-byte store per plane).
@@ -63,30 +41,17 @@ pack_rows_multi_kernel(const __grid_constant__ PackJobs jobs, int B, int H, int 
   const int b = (int)(t % B);
   const int l = (int)(t / B);
   const long long off = t * jb.ld + (long long)h * hd + d;
-  float r[4];
+  float4 r;
   if (HALF_IN) {
     const uint2 raw = __ldg(reinterpret_cast<const uint2 *>(static_cast<const __half *>(jb.src) + off));
     const float2 lo = __half22float2(*reinterpret_cast<const __half2 *>(&raw.x));
     const float2 hi = __half22float2(*reinterpret_cast<const __half2 *>(&raw.y));
-    r[0] = lo.x * jb.scale; r[1] = lo.y * jb.scale; r[2] = hi.x * jb.scale; r[3] = hi.y * jb.scale;
+    r = make_float4(lo.x * jb.scale, lo.y * jb.scale, hi.x * jb.scale, hi.y * jb.scale);
   } else {
     const float4 v = __ldg(reinterpret_cast<const float4 *>(static_cast<const float *>(jb.src) + off));
-    r[0] = v.x * jb.scale; r[1] = v.y * jb.scale; r[2] = v.z * jb.scale; r[3] = v.w * jb.scale;
+    r = make_float4(v.x * jb.scale, v.y * jb.scale, v.z * jb.scale, v.w * jb.scale);
   }
-  __nv_bfloat16 *dst = jb.planes + (((size_t)(b * H + h)) * jb.L + l) * hd + d;
-  const size_t plane_stride = (size_t)total4 * 4;
-#pragma unroll
-  for (int p = 0; p < NSPLIT; ++p) {
-    const __nv_bfloat162 lo = __floats2bfloat162_rn(r[0], r[1]), hi = __floats2bfloat162_rn(r[2], r[3]);
-    uint2 w;
-    w.x = *reinterpret_cast<const uint32_t *>(&lo);
-    w.y = *reinterpret_cast<const uint32_t *>(&hi);
-    *reinterpret_cast<uint2 *>(dst + (size_t)p * plane_stride) = w;
-    if (p + 1 < NSPLIT) {
-      r[0] -= __uint_as_float(w.x << 16); r[1] -= __uint_as_float(w.x & 0xFFFF0000u);
-      r[2] -= __uint_as_float(w.y << 16); r[3] -= __uint_as_float(w.y & 0xFFFF0000u);
-    }
-  }
+  split_store4<NSPLIT>(r, jb.planes + (((size_t)(b * H + h)) * jb.L + l) * hd + d, (size_t)total4 * 4);
 }
 
 // ------------------------------------------------------------------ dropout mask (counter hash)

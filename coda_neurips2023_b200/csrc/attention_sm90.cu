@@ -156,7 +156,7 @@ attn_fwd_kernel(const __grid_constant__ AttnMaps maps, int Lq, int Lk, int B, in
   if (seed_dev) seed += __ldg(seed_dev);  // per-step counter kept on the device (CUDA-graph friendly)
   constexpr int KB = C::KB, NP = p_planes(NSPLIT), NST = C::NST;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  unsigned char *smem = smem_align1024(smem_raw);
   __shared__ __align__(8) uint64_t q_full, kv_full[NST], kv_empty[NST];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -228,11 +228,11 @@ attn_fwd_kernel(const __grid_constant__ AttnMaps maps, int Lq, int Lk, int B, in
     acc_fence(sacc);
     wgmma_fence();
 #pragma unroll
-    for (int p = 0; p < a_nprod(NSPLIT); ++p)
+    for (int p = 0; p < n_products(NSPLIT); ++p)
 #pragma unroll
       for (int kb = 0; kb < KB; ++kb) {
-        const uint64_t ad = gmma_desc_k_sw128(qs + ((a_pa(NSPLIT, p) * NWG) * KB + kb) * C::BOX);
-        const uint64_t bd = gmma_desc_k_sw128(ks + (a_pb(NSPLIT, p) * KB + kb) * C::BOX);
+        const uint64_t ad = gmma_desc_k_sw128(qs + ((prod_a(NSPLIT, p) * NWG) * KB + kb) * C::BOX);
+        const uint64_t bd = gmma_desc_k_sw128(ks + (prod_b(NSPLIT, p) * KB + kb) * C::BOX);
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk)
           Wgmma<KT, F16>::template ss<0, 0>(sacc, gmma_desc_advance(ad, kk * 32), gmma_desc_advance(bd, kk * 32),
@@ -345,15 +345,11 @@ int launch_attn(const AttnMaps &maps, int Lq, int Lk, int B, int H, float *out, 
   // one warpgroup per CTA for short query sequences (the CLIP tower: 50 tokens) and for head dim 128 (its running
   // and per-tile O accumulators take the register file of a one-warpgroup CTA), two otherwise
   const bool one = Lq <= 64 || HD == 128;
-  auto kern = one ? attn_fwd_kernel<HD, NSPLIT, 1, F16> : attn_fwd_kernel<HD, NSPLIT, 2, F16>;
+  constexpr auto kern1 = attn_fwd_kernel<HD, NSPLIT, 1, F16>, kern2 = attn_fwd_kernel<HD, NSPLIT, 2, F16>;
+  const auto kern = one ? kern1 : kern2;
   const int smem = (one ? AttnCfg<HD, NSPLIT, 1>::TOTAL : AttnCfg<HD, NSPLIT, 2>::TOTAL) + 1024;
   const int threads = one ? AttnCfg<HD, NSPLIT, 1>::THREADS : AttnCfg<HD, NSPLIT, 2>::THREADS;
-  static bool configured[2] = {false, false};  // once per template instance
-  if (!configured[one]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return (int)e;
-    configured[one] = true;
-  }
+  if (const int st = one ? raise_smem_limit<kern1>(smem) : raise_smem_limit<kern2>(smem)) return st;
   const int rows = one ? 64 : 128;
   const dim3 grid((Lq + rows - 1) / rows, B * H);
   kern<<<grid, threads, smem, s>>>(maps, Lq, Lk, B, H, out, lse, drop_p, seed, seed_dev, out_half, mask_q);

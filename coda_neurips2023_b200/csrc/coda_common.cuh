@@ -14,6 +14,20 @@ __host__ inline int launch_status() {
   return e == cudaSuccess ? CODA_OK : (int)e;
 }
 
+// Raise kernel Kern's dynamic shared-memory limit to `bytes` on the first call; later calls do nothing, so `bytes` must
+// cover every launch of Kern.  The flag is one per kernel (Kern is the function pointer: the instances of a kernel
+// template share one function type).
+template <auto Kern>
+__host__ inline int raise_smem_limit(int bytes) {
+  static bool done = false;
+  if (!done) {
+    const cudaError_t e = cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e != cudaSuccess) return (int)e;
+    done = true;
+  }
+  return CODA_OK;
+}
+
 __device__ __forceinline__ uint32_t smem_u32(const void *p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }

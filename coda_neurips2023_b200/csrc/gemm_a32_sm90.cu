@@ -21,6 +21,7 @@
 //               tensor pipe works for the other.
 // C-ABI in include/coda_gemm.h (coda_gemm_a32*).
 #include "../../include/coda_gemm.h"
+#include "a32_prologue.cuh"
 #include "sm90_primitives.cuh"
 
 #include <type_traits>
@@ -39,28 +40,6 @@ struct A32Maps {
   CUtensorMap a2;     // second fp32 input of the two-input modes (same geometry)
   CUtensorMap b[3];   // bf16 planes
 };
-
-__host__ __device__ constexpr int n_products(int ns) { return ns == 1 ? 1 : (ns == 2 ? 3 : 6); }
-__host__ __device__ constexpr int prod_a(int ns, int p) {
-  return ns == 1 ? 0 : ns == 2 ? (p == 0 ? 1 : 0) : (p == 0 ? 1 : p == 1 ? 2 : p == 2 ? 0 : p == 3 ? 1 : 0);
-}
-__host__ __device__ constexpr int prod_b(int ns, int p) {
-  return ns == 1 ? 0 : ns == 2 ? (p == 1 ? 1 : 0) : (p == 0 ? 1 : p == 1 ? 0 : p == 2 ? 2 : p == 3 ? 0 : p == 4 ? 1 : 0);
-}
-
-inline int make_tmap_f32_box(CUtensorMap *map, const void *base, long long cols, long long rows, long long row_stride,
-                             int box_cols, int box_rows) {
-  EncodeTiledFn fn = encode_tiled_fn();
-  if (!fn) return CODA_EINVAL;
-  cuuint64_t gdim[3] = {(cuuint64_t)cols, (cuuint64_t)rows, 1};
-  cuuint64_t gstride[2] = {(cuuint64_t)row_stride * 4, (cuuint64_t)row_stride * rows * 4};
-  cuuint32_t box[3] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void *>(base), gdim, gstride, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? CODA_OK : CODA_EINVAL;
-}
 
 struct A32Params {
   int m, n, k;             // k = logical contraction length (A columns); B planes are padded to kpad
@@ -107,7 +86,7 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
   constexpr int B_TILE = BN * BK * 2;
   constexpr int B_STAGE = NSPLIT * B_TILE;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  unsigned char *smem = smem_align1024(smem_raw);
   unsigned char *raw_ring = smem;
   const bool two_in = P.mode == CODA_A32_BN_BWD;
   const bool pooled = P.mode == CODA_A32_BN_BWD_POOLED || P.mode == CODA_A32_BN_BWD_POOLED_PRE;
@@ -278,25 +257,22 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
 #pragma unroll
               for (int i = 0; i < 2; ++i) {
                 float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
-                x.x = fmaxf(fmaf(x.x, s2.x, h2.x), 0.f);
-                x.y = fmaxf(fmaf(x.y, s2.y, h2.y), 0.f);
+                x.x = a32::affine_relu(x.x, s2.x, h2.x);
+                x.y = a32::affine_relu(x.y, s2.y, h2.y);
                 put(i, x);
               }
             } else if (mode == CODA_A32_BN_BWD) {
-              // x = y (pre-BN activation), d = gradient of relu(bn(y)).  With s = gamma * invstd, t = beta_bn - mean * s:
-              //   dy = s * ([s y + t > 0] d - s1/N - xhat s2/N) = [s y + t > 0] * s * d + alpha * y + beta
-              //   alpha = -s * invstd * s2 / N,  beta = -s * s1 / N - alpha * mean        (host: coda_bn_bwd_coefs)
+              // x = y (pre-BN activation), d = gradient of relu(bn(y))
               const float2 s2 = ld2(P.scale), h2 = ld2(P.shift), a2 = ld2(P.alpha), b2 = ld2(P.beta);
 #pragma unroll
               for (int i = 0; i < 2; ++i) {
                 float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
                 const float2 d = *reinterpret_cast<const float2 *>(rt + RAW_TILE + off(i));
-                x.x = (fmaf(x.x, s2.x, h2.x) > 0.f ? s2.x * d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
-                x.y = (fmaf(x.y, s2.y, h2.y) > 0.f ? s2.y * d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
+                x.x = a32::bn_bwd(x.x, d.x, s2.x, h2.x, a2.x, b2.x);
+                x.y = a32::bn_bwd(x.y, d.y, s2.y, h2.y, a2.y, b2.y);
                 put(i, x);
               }
             } else if (mode == CODA_A32_BN_BWD_POOLED_PRE) {
-              // pre-masked, pre-scaled pooled gradient: one compare + select + FMA + add per element
               const unsigned char *px = rt + RAW_TILE + pgt * 320;
               const float2 a2 = ld2(P.alpha), b2 = ld2(P.beta);
               const float2 d = *reinterpret_cast<const float2 *>(px + col * 4);
@@ -305,13 +281,11 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
               for (int i = 0; i < 2; ++i) {
                 float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
                 const int gi = pgi[i];
-                x.x = (id.x == gi ? d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
-                x.y = (id.y == gi ? d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
+                x.x = a32::bn_bwd_pooled_pre(x.x, d.x, id.x == gi, a2.x, b2.x);
+                x.y = a32::bn_bwd_pooled_pre(x.y, d.y, id.y == gi, a2.y, b2.y);
                 put(i, x);
               }
             } else if (mode == CODA_A32_BN_BWD_POOLED) {
-              // the layer output was max-pooled over `group` rows: only the arg-max row of a (group, channel)
-              // carries the incoming gradient dpooled[g][c]
               const unsigned char *px = rt + RAW_TILE + pgt * 320;     // staged by the producer with the raw tile
               const float2 s2 = ld2(P.scale), h2 = ld2(P.shift), a2 = ld2(P.alpha), b2 = ld2(P.beta);
               const float2 d = *reinterpret_cast<const float2 *>(px + col * 4);
@@ -320,8 +294,8 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
               for (int i = 0; i < 2; ++i) {
                 float2 x = *reinterpret_cast<const float2 *>(rt + off(i));
                 const int gi = pgi[i];
-                x.x = ((id.x == gi && fmaf(x.x, s2.x, h2.x) > 0.f) ? s2.x * d.x : 0.f) + fmaf(x.x, a2.x, b2.x);
-                x.y = ((id.y == gi && fmaf(x.y, s2.y, h2.y) > 0.f) ? s2.y * d.y : 0.f) + fmaf(x.y, a2.y, b2.y);
+                x.x = a32::bn_bwd_pooled(x.x, d.x, id.x == gi, s2.x, h2.x, a2.x, b2.x);
+                x.y = a32::bn_bwd_pooled(x.y, d.y, id.y == gi, s2.y, h2.y, a2.y, b2.y);
                 put(i, x);
               }
             } else {
@@ -438,17 +412,6 @@ gemm_a32_kernel(const __grid_constant__ A32Maps maps, const A32Params P) {
   }
 }
 
-int num_sms() {
-  static int n = 0;
-  if (!n) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 132;
-  }
-  return n;
-}
-
 template <int NSPLIT, int BN, int RAW_KB, int B_STAGES, bool B_MN>
 int launch_a32(const A32Maps &maps, const A32Params &P, cudaStream_t s) {
   static_assert(RAW_KB % 64 == 0 || RAW_KB == 96, "raw region");
@@ -457,21 +420,17 @@ int launch_a32(const A32Maps &maps, const A32Params &P, cudaStream_t s) {
   constexpr size_t SMEM_MAX = 227 * 1024 - 2048;     // static shared memory (barriers) shares the 227 KB limit
   if (total > SMEM_MAX) return CODA_ETOOLARGE;
   if (P.mode == CODA_A32_BN_BWD && RAW_KB < 64) return CODA_EINVAL;
-  auto kern = gemm_a32_kernel<NSPLIT, BN, RAW_KB, B_STAGES, B_MN>;
-  static size_t configured = 0;
-  if (configured < total) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_MAX);
-    if (e != cudaSuccess) return (int)e;
-    configured = SMEM_MAX;
-  }
+  constexpr auto kern = gemm_a32_kernel<NSPLIT, BN, RAW_KB, B_STAGES, B_MN>;
+  // the limit covers every launch of the instance, whatever its statistics buffer adds
+  if (const int st = raise_smem_limit<kern>((int)SMEM_MAX)) return st;
   const int tiles_m = (P.m + BM - 1) / BM, tiles_n = (P.n + BN - 1) / BN;
   const long long nwork = (long long)tiles_m * tiles_n;
-  unsigned grid = (unsigned)(nwork < num_sms() ? nwork : num_sms());
+  unsigned grid = (unsigned)(nwork < sm_count() ? nwork : sm_count());
   A32Params Q = P;
   const int nkb = (P.k + BK - 1) / BK;
   // short contraction, many m-tiles: keep the weights of one n-tile resident per CTA
-  Q.b_resident = (nkb <= B_STAGES && tiles_n <= num_sms() && tiles_m >= 4 * (num_sms() / tiles_n)) ? 1 : 0;
-  if (Q.b_resident) grid = (unsigned)((num_sms() / tiles_n) * tiles_n);
+  Q.b_resident = (nkb <= B_STAGES && tiles_n <= sm_count() && tiles_m >= 4 * (sm_count() / tiles_n)) ? 1 : 0;
+  if (Q.b_resident) grid = (unsigned)((sm_count() / tiles_n) * tiles_n);
   kern<<<grid, A32_THREADS, total, s>>>(maps, Q);
   return launch_status();
 }
@@ -483,7 +442,7 @@ extern "C" {
 int coda_gemm_a32_grid(int m, int n) {
   // upper bound of the launch grid = rows of the (zero-initialised) col_stats buffer the caller provides
   if (m <= 0 || n <= 0) return 0;
-  return num_sms();
+  return sm_count();
 }
 
 int coda_gemm_a32(int nsplit, int m, int n, int k, const float *a, long long lda, int a_mode, const float *a_scale,
@@ -506,7 +465,7 @@ int coda_gemm_a32(int nsplit, int m, int n, int k, const float *a, long long lda
   // few output tiles (the decoder's 2048-row linears: 16 x 4 tiles of 128 x 128 on 132 SMs): 64-wide tiles double
   // the number of CTAs at work; each of these launches is bounded by one CTA's serial tile time, not by throughput
   const long long tiles128 = (long long)((m + BM - 1) / BM) * ((n + 127) / 128);
-  const int bn = (n <= 64 || tiles128 <= num_sms() / 2) ? 64 : 128;
+  const int bn = (n <= 64 || tiles128 <= sm_count() / 2) ? 64 : 128;
   A32Maps maps;
   int st = make_tmap_f32_box(&maps.a, a, k, m, lda, 32, BM);
   if (st != CODA_OK) return st;

@@ -21,18 +21,6 @@ using namespace coda;
 namespace {
 
 // ------------------------------------------------------------------ pack (fp32 -> bf16 planes)
-template <int NSPLIT>
-__device__ __forceinline__ void split_store(float x, __nv_bfloat16 *dst, size_t plane_stride) {
-  const __nv_bfloat16 h = __float2bfloat16_rn(x);
-  dst[0] = h;
-  if (NSPLIT >= 2) {
-    const float r1 = x - __bfloat162float(h);
-    const __nv_bfloat16 m = __float2bfloat16_rn(r1);
-    dst[plane_stride] = m;
-    if (NSPLIT >= 3) dst[2 * plane_stride] = __float2bfloat16_rn(r1 - __bfloat162float(m));
-  }
-}
-
 // source is row-major along k (src_k_stride == 1): one thread per (row, k) element, k fastest
 template <int NSPLIT>
 __global__ void __launch_bounds__(256)
@@ -58,20 +46,8 @@ pack_rows_vec4_kernel(long long rows, int k, int kpad, long long src_row_stride,
   const int c = (int)(idx - r * kq) * 4;
   float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
   if (c < k) v = __ldg(reinterpret_cast<const float4 *>(src + r * src_row_stride + c));
-  float x[4] = {v.x * scale, v.y * scale, v.z * scale, v.w * scale};
-  __nv_bfloat16 *dst = planes + r * kpad + c;
-#pragma unroll
-  for (int p = 0; p < NSPLIT; ++p) {
-    const __nv_bfloat162 lo = __floats2bfloat162_rn(x[0], x[1]), hi = __floats2bfloat162_rn(x[2], x[3]);
-    uint2 w;
-    w.x = *reinterpret_cast<const uint32_t *>(&lo);
-    w.y = *reinterpret_cast<const uint32_t *>(&hi);
-    *reinterpret_cast<uint2 *>(dst + (size_t)p * plane_stride) = w;
-    if (p + 1 < NSPLIT) {
-      x[0] -= __uint_as_float(w.x << 16); x[1] -= __uint_as_float(w.x & 0xFFFF0000u);
-      x[2] -= __uint_as_float(w.y << 16); x[3] -= __uint_as_float(w.y & 0xFFFF0000u);
-    }
-  }
+  split_store4<NSPLIT>(make_float4(v.x * scale, v.y * scale, v.z * scale, v.w * scale), planes + r * kpad + c,
+                       (size_t)plane_stride);
 }
 
 // source is contiguous along rows (src_row_stride == 1, "transposed" operand): 32x32 smem transpose
@@ -106,15 +82,6 @@ struct GemmMaps {
   CUtensorMap b[3];
 };
 
-// which (A plane, B plane) pairs are multiplied; small cross terms first
-__host__ __device__ constexpr int n_products(int ns) { return ns == 1 ? 1 : (ns == 2 ? 3 : 6); }
-__host__ __device__ constexpr int prod_a(int ns, int p) {
-  return ns == 1 ? 0 : ns == 2 ? (p == 0 ? 1 : 0) : (p == 0 ? 1 : p == 1 ? 2 : p == 2 ? 0 : p == 3 ? 1 : 0);
-}
-__host__ __device__ constexpr int prod_b(int ns, int p) {
-  return ns == 1 ? 0 : ns == 2 ? (p == 1 ? 1 : 0) : (p == 0 ? 1 : p == 1 ? 0 : p == 2 ? 2 : p == 3 ? 0 : p == 4 ? 1 : 0);
-}
-
 __device__ __forceinline__ float apply_act(float x, int act) {
   if (act == 1) return fmaxf(x, 0.f);
   if (act == 2) return __fdividef(x, 1.0f + __expf(-1.702f * x));
@@ -137,7 +104,7 @@ gemm_nt_kernel(const __grid_constant__ GemmMaps maps, int m, int n, int kpad, in
   constexpr int B_TILE = BN * BK * 2;
   constexpr int STAGE = NSPLIT * (A_TILE + B_TILE);
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  unsigned char *smem = smem_align1024(smem_raw);
   __shared__ __align__(8) uint64_t full_bar[STAGES];
   __shared__ __align__(8) uint64_t empty_bar[STAGES];
 
@@ -331,7 +298,7 @@ gemm_f16_pp_kernel(const __grid_constant__ GemmMaps maps, int m, int n, int nkb,
   constexpr int A_TILE = BM * BK * 2;
   constexpr int STAGE = A_TILE + BN * BK * 2;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  unsigned char *smem = smem_align1024(smem_raw);
   __shared__ __align__(8) uint64_t full_bar[STAGES];
   __shared__ __align__(8) uint64_t empty_bar[STAGES];
 
@@ -448,23 +415,12 @@ gemm_f16_pp_kernel(const __grid_constant__ GemmMaps maps, int m, int n, int nkb,
   }
 }
 
-int device_sms() {
-  static int num_sms = 0;
-  if (!num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (num_sms <= 0) num_sms = 132;
-  }
-  return num_sms;
-}
-
 template <int NSPLIT, int BN, int STAGES, bool FP16, bool MN = false>
 int launch_gemm(const GemmMaps &maps, int batch, int m, int n, int kpad, int b_batched, const float *bias, int relu,
                 void *c_out, long long ldc, long long c_batch_stride, cudaStream_t s, int out_half = 0,
                 const void *residual = nullptr, long long ldr = 0) {
   float *c = reinterpret_cast<float *>(c_out);
-  const int sms = device_sms();
+  const int sms = sm_count();
   // split-K when the output has few tiles but the contraction is long (weight gradients)
   const long long tiles = (long long)((m + BM - 1) / BM) * ((n + BN - 1) / BN) * batch;
   const int nkb_total = kpad / BK;
@@ -486,13 +442,8 @@ int launch_gemm(const GemmMaps &maps, int batch, int m, int n, int kpad, int b_b
   }
   constexpr size_t smem = (size_t)STAGES * NSPLIT * (BM * BK * 2 + BN * BK * 2) + 1024;
   static_assert(smem <= 227 * 1024, "smem budget");
-  auto kern = gemm_nt_kernel<NSPLIT, BN, STAGES, FP16, MN>;
-  static bool configured = false;  // once per template instance
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
+  constexpr auto kern = gemm_nt_kernel<NSPLIT, BN, STAGES, FP16, MN>;
+  if (const int st = raise_smem_limit<kern>((int)smem)) return st;
   const long long nwork = tiles * ksplit;
   const unsigned grid = (unsigned)(nwork < sms ? nwork : sms);
   kern<<<grid, GEMM_THREADS, smem, s>>>(maps, m, n, kpad, b_batched, ksplit, batch, bias, relu, out_half, c_out, ldc,
@@ -511,14 +462,9 @@ int launch_gemm_f16_pp(const GemmMaps &maps, int m, int n, int kpad, const float
                        long long ldr, void *c, long long ldc, cudaStream_t s) {
   constexpr size_t smem = (size_t)STAGES * (BM * BK * 2 + BN * BK * 2) + 1024;
   static_assert(smem <= 227 * 1024, "smem budget");
-  auto kern = gemm_f16_pp_kernel<BN, STAGES, EPI>;
-  static bool configured = false;  // once per template instance
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
-  const int sms = device_sms();
+  constexpr auto kern = gemm_f16_pp_kernel<BN, STAGES, EPI>;
+  if (const int st = raise_smem_limit<kern>((int)smem)) return st;
+  const int sms = sm_count();
   const int tiles = (m + BM - 1) / BM * (n / BN);
   kern<<<(unsigned)(tiles < sms ? tiles : sms), PP_THREADS, smem, s>>>(
       maps, m, n, kpad / BK, bias, reinterpret_cast<const __half *>(residual), ldr, reinterpret_cast<__half *>(c), ldc);
@@ -604,7 +550,7 @@ int coda_gemm_nt_res(int nsplit, int is_fp16, int batch, int m, int n, int kpad,
                      : (relu == 2 && !residual) ? PP_BIAS_GELU : -1;
   const long long pp_tiles = (long long)((m + BM - 1) / BM) * (n / PP_BN);   // int tile indices in the kernel
   const bool pp = is_fp16 && out_half && batch == 1 && pp_epi >= 0 && n % PP_BN == 0 &&
-                  pp_tiles >= 2LL * device_sms() && pp_tiles <= INT_MAX && ldc % 8 == 0 &&
+                  pp_tiles >= 2LL * sm_count() && pp_tiles <= INT_MAX && ldc % 8 == 0 &&
                   ((uintptr_t)c & 15) == 0 && ((uintptr_t)bias & 7) == 0 &&
                   (!residual || (ldr % 8 == 0 && ((uintptr_t)residual & 15) == 0));
   const int bn = pp ? PP_BN

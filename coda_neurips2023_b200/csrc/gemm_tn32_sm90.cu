@@ -18,6 +18,7 @@
 // transform warps on the way -- the values are in registers already -- instead of a separate pass over dY.
 // C-ABI in include/coda_gemm.h (coda_gemm_tn32).
 #include "../../include/coda_gemm.h"
+#include "a32_prologue.cuh"
 #include "sm90_primitives.cuh"
 
 using namespace coda;
@@ -51,22 +52,6 @@ struct TN32Params {
   int ksplit;
 };
 
-__device__ __forceinline__ void store_planes4(float4 v, unsigned char *dst, uint32_t plane_bytes) {
-  float r[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int p = 0; p < NS; ++p) {
-    const __nv_bfloat162 lo = __floats2bfloat162_rn(r[0], r[1]), hi = __floats2bfloat162_rn(r[2], r[3]);
-    uint2 w;
-    w.x = *reinterpret_cast<const uint32_t *>(&lo);
-    w.y = *reinterpret_cast<const uint32_t *>(&hi);
-    *reinterpret_cast<uint2 *>(dst + (size_t)p * plane_bytes) = w;
-    if (p + 1 < NS) {
-      r[0] -= __uint_as_float(w.x << 16); r[1] -= __uint_as_float(w.x & 0xFFFF0000u);
-      r[2] -= __uint_as_float(w.y << 16); r[3] -= __uint_as_float(w.y & 0xFFFF0000u);
-    }
-  }
-}
-
 template <int BN>
 __global__ void __launch_bounds__(TN32_THREADS, 1)
 gemm_tn32_kernel(const __grid_constant__ TN32Maps maps, const TN32Params P) {
@@ -78,7 +63,7 @@ gemm_tn32_kernel(const __grid_constant__ TN32Maps maps, const TN32Params P) {
   constexpr int PL_B = BKR * BN * 2;
   constexpr int PL_STAGE = NS * (PL_A + PL_B);
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  unsigned char *smem = smem_align1024(smem_raw);
   unsigned char *raw_ring = smem;
   unsigned char *pl_ring = smem + (size_t)RAW_STAGES * RAW_STAGE;
   __shared__ __align__(8) uint64_t raw_full[RAW_STAGES], raw_empty[RAW_STAGES];
@@ -185,33 +170,34 @@ gemm_tn32_kernel(const __grid_constant__ TN32Maps maps, const TN32Params P) {
         float4 o = y;
         if (P.a_mode == CODA_A32_BN_BWD) {
           const float4 d = *reinterpret_cast<const float4 *>(raw + RAW_A + roff);
-          o.x = (fmaf(y.x, sa.x, ta.x) > 0.f ? sa.x * d.x : 0.f) + fmaf(y.x, al.x, be.x);
-          o.y = (fmaf(y.y, sa.y, ta.y) > 0.f ? sa.y * d.y : 0.f) + fmaf(y.y, al.y, be.y);
-          o.z = (fmaf(y.z, sa.z, ta.z) > 0.f ? sa.z * d.z : 0.f) + fmaf(y.z, al.z, be.z);
-          o.w = (fmaf(y.w, sa.w, ta.w) > 0.f ? sa.w * d.w : 0.f) + fmaf(y.w, al.w, be.w);
+          o.x = a32::bn_bwd(y.x, d.x, sa.x, ta.x, al.x, be.x);
+          o.y = a32::bn_bwd(y.y, d.y, sa.y, ta.y, al.y, be.y);
+          o.z = a32::bn_bwd(y.z, d.z, sa.z, ta.z, al.z, be.z);
+          o.w = a32::bn_bwd(y.w, d.w, sa.w, ta.w, al.w, be.w);
         } else if (P.a_mode == CODA_A32_BN_BWD_POOLED_PRE) {
           const int gi = rem0 + r;
           const float4 d = *reinterpret_cast<const float4 *>(raw + 2 * RAW_A + RAW_B + lane * 16);
           const uchar4 id = *reinterpret_cast<const uchar4 *>(raw + 2 * RAW_A + RAW_B + 512 + lane * 4);
-          o.x = (id.x == gi ? d.x : 0.f) + fmaf(y.x, al.x, be.x);
-          o.y = (id.y == gi ? d.y : 0.f) + fmaf(y.y, al.y, be.y);
-          o.z = (id.z == gi ? d.z : 0.f) + fmaf(y.z, al.z, be.z);
-          o.w = (id.w == gi ? d.w : 0.f) + fmaf(y.w, al.w, be.w);
+          o.x = a32::bn_bwd_pooled_pre(y.x, d.x, id.x == gi, al.x, be.x);
+          o.y = a32::bn_bwd_pooled_pre(y.y, d.y, id.y == gi, al.y, be.y);
+          o.z = a32::bn_bwd_pooled_pre(y.z, d.z, id.z == gi, al.z, be.z);
+          o.w = a32::bn_bwd_pooled_pre(y.w, d.w, id.w == gi, al.w, be.w);
         } else if (P.a_mode == CODA_A32_BN_BWD_POOLED) {
           const int gi = rem0 + r;
           const float4 d = *reinterpret_cast<const float4 *>(raw + 2 * RAW_A + RAW_B + lane * 16);
           const uchar4 id = *reinterpret_cast<const uchar4 *>(raw + 2 * RAW_A + RAW_B + 512 + lane * 4);
-          o.x = ((id.x == gi && fmaf(y.x, sa.x, ta.x) > 0.f) ? sa.x * d.x : 0.f) + fmaf(y.x, al.x, be.x);
-          o.y = ((id.y == gi && fmaf(y.y, sa.y, ta.y) > 0.f) ? sa.y * d.y : 0.f) + fmaf(y.y, al.y, be.y);
-          o.z = ((id.z == gi && fmaf(y.z, sa.z, ta.z) > 0.f) ? sa.z * d.z : 0.f) + fmaf(y.z, al.z, be.z);
-          o.w = ((id.w == gi && fmaf(y.w, sa.w, ta.w) > 0.f) ? sa.w * d.w : 0.f) + fmaf(y.w, al.w, be.w);
+          o.x = a32::bn_bwd_pooled(y.x, d.x, id.x == gi, sa.x, ta.x, al.x, be.x);
+          o.y = a32::bn_bwd_pooled(y.y, d.y, id.y == gi, sa.y, ta.y, al.y, be.y);
+          o.z = a32::bn_bwd_pooled(y.z, d.z, id.z == gi, sa.z, ta.z, al.z, be.z);
+          o.w = a32::bn_bwd_pooled(y.w, d.w, id.w == gi, sa.w, ta.w, al.w, be.w);
         }
         if (tail && grow >= P.rows) o = make_float4(0.f, 0.f, 0.f, 0.f);     // padding rows of the last slab
         if (want_colsum) { csum.x += o.x; csum.y += o.y; csum.z += o.z; csum.w += o.w; }
         // destination: box = column / 64, 16-byte chunk = (column % 64) / 8 swizzled by the row, half = (column % 8) / 4
         const int col = lane * 4;
-        store_planes4(o, pl + (col >> 6) * (BKR * 128) + r * 128 + ((((col & 63) >> 3) ^ (r & 7)) << 4) + ((col & 7) >> 2) * 8,
-                      PL_A);
+        split_store4<NS>(o, reinterpret_cast<__nv_bfloat16 *>(pl + (col >> 6) * (BKR * 128) + r * 128 +
+                                                              ((((col & 63) >> 3) ^ (r & 7)) << 4) + ((col & 7) >> 2) * 8),
+                         PL_A / 2);
       }
       // ---- B slab
 #pragma unroll
@@ -221,27 +207,26 @@ gemm_tn32_kernel(const __grid_constant__ TN32Maps maps, const TN32Params P) {
         const uint32_t roff = (uint32_t)(bch >> 3) * 4096u + (uint32_t)r * 128u + (uint32_t)(((bch & 7) ^ (r & 7)) << 4);
         float4 v = *reinterpret_cast<const float4 *>(raw + 2 * RAW_A + roff);
         if (P.b_mode == CODA_A32_AFFINE_RELU) {
-          v.x = fmaxf(fmaf(v.x, sb.x, tb.x), 0.f); v.y = fmaxf(fmaf(v.y, sb.y, tb.y), 0.f);
-          v.z = fmaxf(fmaf(v.z, sb.z, tb.z), 0.f); v.w = fmaxf(fmaf(v.w, sb.w, tb.w), 0.f);
+          v.x = a32::affine_relu(v.x, sb.x, tb.x); v.y = a32::affine_relu(v.y, sb.y, tb.y);
+          v.z = a32::affine_relu(v.z, sb.z, tb.z); v.w = a32::affine_relu(v.w, sb.w, tb.w);
         }
         if (tail && grow >= P.rows) v = make_float4(0.f, 0.f, 0.f, 0.f);
         const int col = bch * 4;
-        store_planes4(v, pl + NS * PL_A + (col >> 6) * (BKR * 128) + r * 128 + ((((col & 63) >> 3) ^ (r & 7)) << 4) +
-                             ((col & 7) >> 2) * 8,
-                      PL_B);
+        split_store4<NS>(v, reinterpret_cast<__nv_bfloat16 *>(pl + NS * PL_A + (col >> 6) * (BKR * 128) + r * 128 +
+                                                              ((((col & 63) >> 3) ^ (r & 7)) << 4) + ((col & 7) >> 2) * 8),
+                         PL_B / 2);
       }
       fence_proxy_async_smem();      // generic-proxy writes -> visible to the tensor core's async-proxy reads
       __syncwarp();
       if (lane == 0) mbar_arrive(&raw_empty[rs]);
       bar_sync(1, 256);              // both operand slabs are complete in shared memory
-      // plane products: lo*hi, hi*lo, hi*hi (small terms first); the warpgroup's 64 rows are the A slab's box wg
+      // plane products; the warpgroup's 64 rows are the A slab's box wg
       acc_fence(acc);
       wgmma_fence();
 #pragma unroll
-      for (int p = 0; p < 3; ++p) {
-        const int pa = p == 0 ? 1 : 0, pb = p == 1 ? 1 : 0;
-        const uint64_t ad = gmma_desc_mn_sw128(pl + pa * PL_A + wg * (BKR * 128), BKR * 128);
-        const uint64_t bd = gmma_desc_mn_sw128(pl + NS * PL_A + pb * PL_B, BKR * 128);
+      for (int p = 0; p < n_products(NS); ++p) {
+        const uint64_t ad = gmma_desc_mn_sw128(pl + prod_a(NS, p) * PL_A + wg * (BKR * 128), BKR * 128);
+        const uint64_t bd = gmma_desc_mn_sw128(pl + NS * PL_A + prod_b(NS, p) * PL_B, BKR * 128);
 #pragma unroll
         for (int kk = 0; kk < BKR / 16; ++kk)
           Wgmma<BN, false>::template ss<1, 1>(acc, gmma_desc_advance(ad, kk * 16 * 128), gmma_desc_advance(bd, kk * 16 * 128),
@@ -301,39 +286,14 @@ colsum_reduce_kernel(const float *__restrict__ parts, int ksplit, int m, float *
   a_colsum[col] = v;
 }
 
-inline int make_tmap_f32_box(CUtensorMap *map, const void *base, long long cols, long long rows, long long row_stride,
-                             int box_cols, int box_rows) {
-  EncodeTiledFn fn = encode_tiled_fn();
-  if (!fn) return CODA_EINVAL;
-  cuuint64_t gdim[3] = {(cuuint64_t)cols, (cuuint64_t)rows, 1};
-  cuuint64_t gstride[2] = {(cuuint64_t)row_stride * 4, (cuuint64_t)row_stride * rows * 4};
-  cuuint32_t box[3] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void *>(base), gdim, gstride, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? CODA_OK : CODA_EINVAL;
-}
-
 template <int BN>
 int launch_tn32(const TN32Maps &maps, TN32Params P, float *c, long long ldc, cudaStream_t s) {
   constexpr size_t smem = (size_t)RAW_STAGES * (2 * BKR * BM * 4 + BKR * BN * 4 + 1024) +
                           (size_t)PL_STAGES * NS * (BKR * BM * 2 + BKR * BN * 2) + 1024;
   static_assert(smem <= 227 * 1024, "smem budget");
-  auto kern = gemm_tn32_kernel<BN>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
-  static int num_sms = 0;
-  if (!num_sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (num_sms <= 0) num_sms = 132;
-  }
+  constexpr auto kern = gemm_tn32_kernel<BN>;
+  if (const int st = raise_smem_limit<kern>((int)smem)) return st;
+  const int num_sms = sm_count();
   const int tiles = ((P.m + BM - 1) / BM) * ((P.n + BN - 1) / BN);
   const long long nkb_total = (P.rows + BKR - 1) / BKR;
   int ksplit = num_sms / tiles;

@@ -226,13 +226,9 @@ template <typename OutT>
 int launch_crop(const CropPlan &p, int h, int w, int ncrops, int res, int patch, const uchar4 *rgbx, const int *scene,
                 const int *boxes, const unsigned char *valid, const float *mean, const float *std, OutT *out,
                 cudaStream_t s) {
-  auto kern = crop_resize_sep_kernel<OutT>;
-  static size_t configured = 0;
-  if (configured < p.smem) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CR_SMEM_LIMIT);
-    if (e != cudaSuccess) return (int)e;
-    configured = CR_SMEM_LIMIT;
-  }
+  constexpr auto kern = crop_resize_sep_kernel<OutT>;
+  // crop_plan keeps every launch within CR_SMEM_LIMIT
+  if (const int st = raise_smem_limit<kern>((int)CR_SMEM_LIMIT)) return st;
   const dim3 grid((res + p.tr - 1) / p.tr, ncrops);
   kern<<<grid, CR_THREADS, p.smem, s>>>(h, w, res, p.tr, p.rmax, p.xt, p.yt, patch, rgbx, scene, boxes, valid, mean[0],
                                         mean[1], mean[2], std[0], std[1], std[2], out);

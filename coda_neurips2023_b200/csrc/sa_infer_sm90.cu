@@ -47,9 +47,6 @@ constexpr int POOL_FLOATS = 2 * 2 * 4 * 128;               // [warpgroup][half][
 // layer-3 plane products (A plane, B plane), smallest terms first
 __host__ __device__ constexpr int l3_a(int p) { return p == 0 ? 1 : p == 1 ? 2 : p == 2 ? 1 : 0; }
 __host__ __device__ constexpr int l3_b(int p) { return p == 0 ? 1 : p == 1 ? 0 : p == 2 ? 0 : p == 3 ? 1 : 0; }
-// layer-2 plane products, 3 x 3 planes (as the training GEMMs, gemm_a32_sm90.cu)
-__host__ __device__ constexpr int l2_a(int p) { return p == 0 ? 1 : p == 1 ? 2 : p == 2 ? 0 : p == 3 ? 1 : 0; }
-__host__ __device__ constexpr int l2_b(int p) { return p == 0 ? 1 : p == 1 ? 0 : p == 2 ? 2 : p == 3 ? 0 : p == 4 ? 1 : 0; }
 
 struct InferMaps {
   CUtensorMap w2[W2_PLANES];   // [128 rows][64 k] per plane, box [128][64]
@@ -71,7 +68,7 @@ template <int C0>
 __global__ void __launch_bounds__(THREADS, 1)
 sa_infer_kernel(const __grid_constant__ InferMaps maps, const InferParams P) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  unsigned char *smem = smem_align1024(smem_raw);
   unsigned char *w2s = smem;
   unsigned char *w3s = smem + SMEM_W2;                       // [plane][k-block] tiles
   float *w1s = reinterpret_cast<float *>(w3s + SMEM_W3);     // [C0][64]: a thread's column pair is one float2
@@ -155,16 +152,16 @@ sa_infer_kernel(const __grid_constant__ InferMaps maps, const InferParams P) {
     // the next seed's input is in flight during this seed's tensor-core work
     if (s + step < P.seeds) load_x(s + step);
 
-    // ---- layer 2: 64 x 128 x 64, six plane products
+    // ---- layer 2: 64 x 128 x 64, the six plane products of 3 x 3 planes
     float acc2[C2 / 2];
     acc_fence(acc2);
     wgmma_fence();
 #pragma unroll
-    for (int p = 0; p < 6; ++p) {
-      const uint64_t bd = gmma_desc_k_sw128(w2s + l2_b(p) * W2_TILE);
+    for (int p = 0; p < n_products(3); ++p) {
+      const uint64_t bd = gmma_desc_k_sw128(w2s + prod_b(3, p) * W2_TILE);
 #pragma unroll
       for (int kk = 0; kk < C1 / 16; ++kk)
-        Wgmma<128, false>::template rs<0>(acc2, a2f[kk][l2_a(p)], gmma_desc_advance(bd, kk * 32), (p | kk) != 0);
+        Wgmma<128, false>::template rs<0>(acc2, a2f[kk][prod_a(3, p)], gmma_desc_advance(bd, kk * 32), (p | kk) != 0);
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -230,30 +227,14 @@ sa_infer_kernel(const __grid_constant__ InferMaps maps, const InferParams P) {
   }
 }
 
-int num_sms() {
-  static int n = 0;
-  if (!n) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 132;
-  }
-  return n;
-}
-
 template <int C0>
 int launch_infer(const InferMaps &maps, const InferParams &P, cudaStream_t s) {
   constexpr size_t smem = 1024 + SMEM_W2 + SMEM_W3 + (size_t)(C0 * C1 + AFFINE_FLOATS + POOL_FLOATS) * 4;
   static_assert(smem <= 227 * 1024 - 1024, "shared memory");
-  auto kern = sa_infer_kernel<C0>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
+  constexpr auto kern = sa_infer_kernel<C0>;
+  if (const int st = raise_smem_limit<kern>((int)smem)) return st;
   const long long pairs = (P.seeds + 1) / 2;
-  const unsigned grid = (unsigned)(pairs < num_sms() ? pairs : num_sms());
+  const unsigned grid = (unsigned)(pairs < sm_count() ? pairs : sm_count());
   kern<<<grid, THREADS, smem, s>>>(maps, P);
   return launch_status();
 }

@@ -12,6 +12,7 @@
 
 #include "../../include/coda_sa_mlp.h"
 #include "coda_common.cuh"
+#include "operand_split.cuh"
 
 namespace {
 
@@ -45,24 +46,6 @@ __device__ __forceinline__ float4 xhat4(const float4 v, const Affine4 &a) {
 __device__ __forceinline__ float4 bn4(const float4 xh, const Affine4 &a) {
   return make_float4(xh.x * a.gamma.x + a.beta.x, xh.y * a.gamma.y + a.beta.y, xh.z * a.gamma.z + a.beta.z,
                      xh.w * a.gamma.w + a.beta.w);
-}
-
-// four values -> NS bf16 planes, 8 bytes per plane
-template <int NS>
-__device__ __forceinline__ void store_planes4(float4 v, __nv_bfloat16 *dst, size_t plane_stride) {
-  float r[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int p = 0; p < NS; ++p) {
-    const __nv_bfloat162 lo = __floats2bfloat162_rn(r[0], r[1]), hi = __floats2bfloat162_rn(r[2], r[3]);
-    uint2 w;
-    w.x = *reinterpret_cast<const uint32_t *>(&lo);
-    w.y = *reinterpret_cast<const uint32_t *>(&hi);
-    *reinterpret_cast<uint2 *>(dst + (size_t)p * plane_stride) = w;
-    if (p + 1 < NS) {
-      r[0] -= __uint_as_float(w.x << 16); r[1] -= __uint_as_float(w.x & 0xFFFF0000u);
-      r[2] -= __uint_as_float(w.y << 16); r[3] -= __uint_as_float(w.y & 0xFFFF0000u);
-    }
-  }
 }
 
 // block-level sum of NV float4 accumulators over the row slots; thread (slot 0, c4) ends with the total
@@ -289,8 +272,8 @@ bn_relu_pack_kernel(long long rows, int c, const float *__restrict__ y, const fl
   const size_t plane_stride = (size_t)rows * c;
   for (long long r = (long long)blockIdx.x * nslots + slot; r < rows; r += (long long)gridDim.x * nslots) {
     const float4 z = bn4(xhat4(__ldg(reinterpret_cast<const float4 *>(y + r * c) + c4), a), a);
-    store_planes4<NS>(make_float4(fmaxf(z.x, 0.f), fmaxf(z.y, 0.f), fmaxf(z.z, 0.f), fmaxf(z.w, 0.f)),
-                      planes + r * c + c4 * 4, plane_stride);
+    coda::split_store4<NS>(make_float4(fmaxf(z.x, 0.f), fmaxf(z.y, 0.f), fmaxf(z.z, 0.f), fmaxf(z.w, 0.f)),
+                           planes + r * c + c4 * 4, plane_stride);
   }
 }
 
@@ -450,7 +433,7 @@ bn_relu_bwd_pack_kernel(long long rows, int c, const float *__restrict__ y, cons
       d = __ldg(reinterpret_cast<const float4 *>(dz + r * c) + c4);
     }
     d.x = z.x > 0.f ? d.x : 0.f; d.y = z.y > 0.f ? d.y : 0.f; d.z = z.z > 0.f ? d.z : 0.f; d.w = z.w > 0.f ? d.w : 0.f;
-    store_planes4<NS>(dy4(d, xh, q), planes + r * c + c4 * 4, plane_stride);
+    coda::split_store4<NS>(dy4(d, xh, q), planes + r * c + c4 * 4, plane_stride);
   }
 }
 

@@ -1,5 +1,6 @@
-// Hopper (sm_90a) building blocks shared by the tensor-core kernels: TMA tensor-map encoding (host), TMA loads and
-// stores, wgmma fences / groups and shared-memory operand descriptors.  Inline PTX only.
+// Hopper (sm_90a) building blocks shared by the tensor-core kernels: TMA tensor-map encoding, the SM count and
+// split-K scratch (host); TMA loads and stores, wgmma fences / groups and shared-memory operand descriptors (inline
+// PTX).  The bf16 operand-plane format comes with it from operand_split.cuh.
 #pragma once
 #include <cuda.h>  // CUtensorMap types (header only; the driver entry point is fetched at run time)
 #include <cuda_bf16.h>
@@ -8,6 +9,7 @@
 #include <mutex>
 
 #include "coda_common.cuh"
+#include "operand_split.cuh"
 #include "wgmma_ops.cuh"
 
 namespace coda {
@@ -51,6 +53,36 @@ inline int make_tmap_k_major_16b(CUtensorMap *map, const void *base, int is_fp16
                   const_cast<void *>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? CODA_OK : CODA_EINVAL;
+}
+
+// fp32 matrix [rows][cols] with row stride `row_stride` (elements), box = [box_rows][box_cols], 128-byte swizzle
+// (box_cols = 32: one swizzle span of fp32)
+inline int make_tmap_f32_box(CUtensorMap *map, const void *base, long long cols, long long rows, long long row_stride,
+                             int box_cols, int box_rows) {
+  EncodeTiledFn fn = encode_tiled_fn();
+  if (!fn) return CODA_EINVAL;
+  cuuint64_t gdim[3] = {(cuuint64_t)cols, (cuuint64_t)rows, 1};
+  cuuint64_t gstride[2] = {(cuuint64_t)row_stride * 4, (cuuint64_t)row_stride * rows * 4};
+  cuuint32_t box[3] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void *>(base), gdim, gstride, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? CODA_OK : CODA_EINVAL;
+}
+
+// --------------------------------------------------------------------- host: launch geometry
+// SMs of the device current at the first call, kept for later calls; 132 (an H100 SXM) if the query fails.
+// Persistent grids and split-K factors are sized from it.
+inline int sm_count() {
+  static int n = 0;
+  if (!n) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    if (n <= 0) n = 132;
+  }
+  return n;
 }
 
 // --------------------------------------------------------------------- host: split-K scratch
@@ -191,29 +223,10 @@ __device__ __forceinline__ uint64_t gmma_desc_mn_sw128(const void *tile, uint32_
 // advance the start address by `bytes` (K-major: k-steps of 32 B inside the swizzle atom; MN-major: 16 rows)
 __device__ __forceinline__ uint64_t gmma_desc_advance(uint64_t desc, uint32_t bytes) { return desc + (bytes >> 4); }
 
-// two floats -> one register of two 16-bit values (low half = first), bf16 or IEEE half
-template <bool F16>
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  if constexpr (F16) {
-    const __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<const uint32_t *>(&h);
-  } else {
-    const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<const uint32_t *>(&h);
-  }
-}
-// a pair of values -> NP bf16 planes (plane p = bf16 rounding of what the previous planes left over)
-template <int NP>
-__device__ __forceinline__ void split_pair(float r0, float r1, uint32_t (&w)[NP]) {
-#pragma unroll
-  for (int p = 0; p < NP; ++p) {
-    const uint32_t bits = pack2<false>(r0, r1);
-    w[p] = bits;
-    if (p + 1 < NP) {
-      r0 -= __uint_as_float(bits << 16);
-      r1 -= __uint_as_float(bits & 0xFFFF0000u);
-    }
-  }
+// The dynamic shared-memory base rounded up to 1024 bytes, the alignment of 128B-swizzled TMA boxes and wgmma tiles
+// (launches request 1024 bytes more than their layout uses).
+__device__ __forceinline__ unsigned char *smem_align1024(unsigned char *smem_raw) {
+  return reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
 }
 
 }  // namespace coda

@@ -80,7 +80,8 @@ int coda_gemm_tn(int nsplit, int mc, int m, int n, const void *a, long long a_pl
  *
  * A is read as fp32 rows (row stride lda, multiple of 4 elements, 16-byte aligned base) by TMA, transformed
  * element-wise by T, split into `nsplit` (2 or 3) bf16 planes and handed to the tensor cores as register
- * operands -- no packed copy of A exists in HBM.  T (`a_mode`), with per-k vectors padded to a multiple of 64:
+ * operands -- no packed copy of A exists in HBM.  T (`a_mode`), with per-k vectors padded to a multiple of 64 (the
+ * element formulas, shared with coda_gemm_tn32, are in csrc/a32_prologue.cuh):
  *   CODA_A32_PLAIN          T = a                                   (every nn.Linear / 1x1 conv on the path)
  *   CODA_A32_AFFINE_RELU    T = relu(a * scale[k] + shift[k])       (BatchNorm(batch stats) + ReLU of the previous
  *                                                                    layer: pytorch_utils.py:8-33 SharedMLP blocks)
