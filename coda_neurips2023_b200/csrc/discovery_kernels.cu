@@ -154,30 +154,91 @@ int coda_novel_candidates(int b, int q, int g, int cap, const int *boxes2d, cons
 
 // ---------------------------------------------------------------------------------------------------------------
 // Predicted 3-D boxes -> 2-D boxes in the image (one thread per box, fp64 like the reference):
-//   undo the point-cloud augmentation (scale, rotation, flips), rotate into the camera frame (Rtilt^T), project with
-//   K, clip to the original image, add the crop offsets, undo the image flip, then the integer bounding box of the
-//   eight projected corners (truncation of non-negative values, as `int(torch.min(.))`) and the usability flag.
-// Replaces models/model_3detr.py:912-968 + datasets/sunrgbd_utils.py:611-635 (project_3dpoint_to_2dpoint_corners_tensor)
-// + the per-box checks of :1034-1051 -- in the reference a chain of fp64 tensor ops plus four .item() syncs per box.
+//   undo the point-cloud augmentation (scale, rotation, flips), move into the camera frame and project, clip to the
+//   original image, add the crop offsets, undo the image flip, then the integer bounding box of the eight projected
+//   corners (truncation of non-negative values, as `int(torch.min(.))`) and the usability flag.
+// Replaces models/model_3detr.py:912-968 + the per-box checks of :1034-1051 -- in the reference a chain of fp64
+// tensor ops plus four .item() syncs per box -- with the camera model of the dataset:
+//   SUN RGB-D (datasets/sunrgbd_utils.py:611-635): Rtilt^T p, depth -> camera axis swap, K (3x3) p.
+//   ScanNet   (datasets/scannet_utils.py:650-690): inv(pose) [p, 1] with the 4x4 camera-to-world pose, K[:3,:3] p.
 namespace {
 
-__global__ void __launch_bounds__(128)
-boxes_in_image_kernel(int b, int q, const float *__restrict__ corners, const float *__restrict__ size,
+constexpr int BII_THREADS = 128;
+
+// inv(A) of a row-major 4x4 fp64 matrix: Gauss-Jordan elimination with partial pivoting (the row of the largest
+// |entry| in the column, first one on ties), like the LU with partial pivoting behind torch.linalg.inv.  Every loop
+// bound is a constant, so the augmented matrix stays in registers.  Returns false for a singular matrix.
+__device__ bool invert4_partial_pivot(const double *__restrict__ A, double *__restrict__ out) {
+  double m[4][8];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) { m[r][c] = A[4 * r + c]; m[r][4 + c] = (r == c) ? 1.0 : 0.0; }
+  bool ok = true;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    int p = k;
+    double best = fabs(m[k][k]);
+#pragma unroll
+    for (int r = k + 1; r < 4; ++r)
+      if (fabs(m[r][k]) > best) { best = fabs(m[r][k]); p = r; }
+#pragma unroll
+    for (int r = k + 1; r < 4; ++r)
+      if (p == r) {
+#pragma unroll
+        for (int c = 0; c < 8; ++c) { const double t = m[k][c]; m[k][c] = m[r][c]; m[r][c] = t; }
+      }
+    ok = ok && best > 0.0;
+    const double inv = 1.0 / m[k][k];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) m[k][c] *= inv;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      if (r == k) continue;
+      const double f = m[r][k];
+#pragma unroll
+      for (int c = 0; c < 8; ++c) m[r][c] -= f * m[k][c];
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) out[4 * r + c] = m[r][4 + c];
+  return ok;
+}
+
+__global__ void __launch_bounds__(BII_THREADS)
+boxes_in_image_kernel(int b, int q, int camera, const float *__restrict__ corners, const float *__restrict__ size,
                       const double *__restrict__ scale, const double *__restrict__ rot, const double *__restrict__ flip,
                       const double *__restrict__ zx_flip, const double *__restrict__ Kmat,
                       const double *__restrict__ Rtilt, const long long *__restrict__ ori_w,
                       const long long *__restrict__ ori_h, const long long *__restrict__ x_off,
                       const long long *__restrict__ y_off, const double *__restrict__ img_flip,
-                      const double *__restrict__ flip_len, int *__restrict__ boxes, unsigned char *__restrict__ valid) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+                      const double *__restrict__ flip_len, int *__restrict__ boxes, unsigned char *__restrict__ valid,
+                      double *__restrict__ extent) {
+  // ScanNet: the inverse pose of every scene this block touches, computed once per scene, so that every box of a
+  // scene is projected with the same matrix
+  __shared__ double pose_inv[BII_THREADS][16];
+  __shared__ unsigned char pose_ok[BII_THREADS];
+  const int first = blockIdx.x * BII_THREADS;
+  const int s0 = first / q;
+  if (camera == CODA_CAMERA_SCANNET) {
+    const int s1 = min(first + BII_THREADS, b * q) - 1;
+    const int ns = s1 / q - s0 + 1;                        // <= BII_THREADS: a block holds at most that many boxes
+    if ((int)threadIdx.x < ns)
+      pose_ok[threadIdx.x] = invert4_partial_pivot(Rtilt + (size_t)(s0 + threadIdx.x) * 16, pose_inv[threadIdx.x]);
+    __syncthreads();
+  }
+  const int i = first + threadIdx.x;
   if (i >= b * q) return;
   const int s = i / q;
-  const double *R = rot + s * 9, *T = Rtilt + s * 9, *K = Kmat + s * 9, *sc = scale + s * 3;
+  const double *R = rot + s * 9, *sc = scale + s * 3;
   const double fx = flip[s], zx = zx_flip ? zx_flip[s] : 1.0;
   const double wmax = (double)(ori_w[s] - 1), hmax = (double)(ori_h[s] - 1);
   const double yo = (double)y_off[s], xo = (double)x_off[s], fl = img_flip[s], flen = flip_len[s];
   double umin = 1e300, vmin = 1e300, umax = -1e300, vmax = -1e300, dmin = 1e300;
   const float *c = corners + (size_t)i * 24;
+  bool pose_good = true;
   for (int k = 0; k < 8; ++k) {
     const double p0 = (double)c[k * 3] * sc[0], p1 = (double)c[k * 3 + 1] * sc[1], p2 = (double)c[k * 3 + 2] * sc[2];
     double r0 = p0 * R[0] + p1 * R[3] + p2 * R[6];      // row vector times rot_array
@@ -185,13 +246,26 @@ boxes_in_image_kernel(int b, int q, const float *__restrict__ corners, const flo
     const double r2 = p0 * R[2] + p1 * R[5] + p2 * R[8];
     r1 *= zx;
     r0 *= fx;
-    const double t0 = T[0] * r0 + T[3] * r1 + T[6] * r2;   // Rtilt^T p
-    const double t1 = T[1] * r0 + T[4] * r1 + T[7] * r2;
-    const double t2 = T[2] * r0 + T[5] * r1 + T[8] * r2;
-    const double c0 = t0, c1 = -t2, c2 = t1;               // depth -> camera axes
-    const double u3 = c0 * K[0] + c1 * K[1] + c2 * K[2];
-    const double v3 = c0 * K[3] + c1 * K[4] + c2 * K[5];
-    const double d = c0 * K[6] + c1 * K[7] + c2 * K[8];
+    double u3, v3, d;
+    if (camera == CODA_CAMERA_SCANNET) {
+      const double *P = pose_inv[s - s0], *K = Kmat + s * 16;
+      pose_good = pose_ok[s - s0] != 0;
+      const double c0 = P[0] * r0 + P[1] * r1 + P[2] * r2 + P[3];     // inv(pose) [p, 1], rows 0..2
+      const double c1 = P[4] * r0 + P[5] * r1 + P[6] * r2 + P[7];
+      const double c2 = P[8] * r0 + P[9] * r1 + P[10] * r2 + P[11];
+      u3 = K[0] * c0 + K[1] * c1 + K[2] * c2;                            // K[:3, :3] p_cam
+      v3 = K[4] * c0 + K[5] * c1 + K[6] * c2;
+      d = K[8] * c0 + K[9] * c1 + K[10] * c2;
+    } else {
+      const double *T = Rtilt + s * 9, *K = Kmat + s * 9;
+      const double t0 = T[0] * r0 + T[3] * r1 + T[6] * r2;   // Rtilt^T p
+      const double t1 = T[1] * r0 + T[4] * r1 + T[7] * r2;
+      const double t2 = T[2] * r0 + T[5] * r1 + T[8] * r2;
+      const double c0 = t0, c1 = -t2, c2 = t1;               // depth -> camera axes
+      u3 = c0 * K[0] + c1 * K[1] + c2 * K[2];
+      v3 = c0 * K[3] + c1 * K[4] + c2 * K[5];
+      d = c0 * K[6] + c1 * K[7] + c2 * K[8];
+    }
     double u = u3 / (d + 1e-32), v = v3 / (d + 1e-32);
     u = fmin(fmax(u, 0.0), wmax) + yo;
     v = fmin(fmax(v, 0.0), hmax) + xo;
@@ -202,24 +276,26 @@ boxes_in_image_kernel(int b, int q, const float *__restrict__ corners, const flo
   }
   const int xmin = (int)umin, ymin = (int)vmin, xmax = (int)umax, ymax = (int)vmax;
   boxes[4 * i] = xmin; boxes[4 * i + 1] = ymin; boxes[4 * i + 2] = xmax; boxes[4 * i + 3] = ymax;
+  if (extent) { extent[4 * i] = umin; extent[4 * i + 1] = vmin; extent[4 * i + 2] = umax; extent[4 * i + 3] = vmax; }
   const float smax = fmaxf(size[3 * i], fmaxf(size[3 * i + 1], size[3 * i + 2]));
-  valid[i] = ((xmax - xmin) > 0 && (ymax - ymin) > 0 && dmin >= 0.0 && !(smax < 1e-16f)) ? 1 : 0;
+  valid[i] = (pose_good && (xmax - xmin) > 0 && (ymax - ymin) > 0 && dmin >= 0.0 && !(smax < 1e-16f)) ? 1 : 0;
 }
 
 }  // namespace
 
-extern "C" int coda_boxes_in_image(int b, int q, const float *corners_xyz, const float *size_unnorm,
+extern "C" int coda_boxes_in_image(int b, int q, int camera, const float *corners_xyz, const float *size_unnorm,
                                    const double *scale, const double *rot, const double *flip, const double *zx_flip,
                                    const double *K, const double *Rtilt, const long long *ori_w, const long long *ori_h,
                                    const long long *x_off, const long long *y_off, const double *img_flip,
-                                   const double *flip_len, int *boxes, unsigned char *valid, void *stream) {
-  if (b < 0 || q < 0) return CODA_EINVAL;
+                                   const double *flip_len, int *boxes, unsigned char *valid, double *extent,
+                                   void *stream) {
+  if (b < 0 || q < 0 || (camera != CODA_CAMERA_SUNRGBD && camera != CODA_CAMERA_SCANNET)) return CODA_EINVAL;
   if (b == 0 || q == 0) return CODA_OK;
   if (!corners_xyz || !size_unnorm || !scale || !rot || !flip || !K || !Rtilt || !ori_w || !ori_h || !x_off || !y_off ||
       !img_flip || !flip_len || !boxes || !valid)
     return CODA_EINVAL;
-  boxes_in_image_kernel<<<(b * q + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
-      b, q, corners_xyz, size_unnorm, scale, rot, flip, zx_flip, K, Rtilt, ori_w, ori_h, x_off, y_off, img_flip, flip_len,
-      boxes, valid);
+  boxes_in_image_kernel<<<(b * q + BII_THREADS - 1) / BII_THREADS, BII_THREADS, 0, (cudaStream_t)stream>>>(
+      b, q, camera, corners_xyz, size_unnorm, scale, rot, flip, zx_flip, K, Rtilt, ori_w, ori_h, x_off, y_off, img_flip,
+      flip_len, boxes, valid, extent);
   return launch_status();
 }

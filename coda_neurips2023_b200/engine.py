@@ -356,6 +356,12 @@ class TrainStep:
             for t, saved in snap:
                 t.copy_(saved)
 
+    def _drop_dry_run_pseudo_labels(self):
+        """Stage-2 discovery rows of a probe or warm-up step are not a step's result: they are dropped instead of
+        being written to the scenes' files (the next discovery step would flush them, inside a graph capture too)."""
+        if getattr(self.model, "_pending_pseudo", None) is not None:
+            self.model._pending_pseudo = None
+
     # ------------------------------------------------------------------ preparation
     def prepare(self, example_batch: dict):
         if self.flat is not None:
@@ -387,6 +393,7 @@ class TrainStep:
         for h in handles:
             h.remove()
         self._restore(snap)
+        self._drop_dry_run_pseudo_labels()
         inactive = [p for _, p in named if id(p) not in fired]
         if is_distributed() and self.world > 1:
             # every rank must lay the buffers out identically: compare the ready order with rank 0's
@@ -440,6 +447,7 @@ class TrainStep:
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
         self._restore(snap)
+        self._drop_dry_run_pseudo_labels()
         self._draw_selection(bsz)
         ops.invalidate_weight_cache()
         from . import _lib

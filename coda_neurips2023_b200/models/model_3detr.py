@@ -42,6 +42,8 @@ CLIP_CHECKPOINT = "./CLIP/pretrain_models/ViT-B-16.pt"  # path the reference har
 ALL_CLASS_PATH_V1 = "datasets/all_classes_trainval_v1.npy"
 ALL_CLASS_PATH_V2 = "datasets/all_classes_trainval_v2_revised_del_val_less_than_5_classes.npy"
 ALL_SUPERCLASS_PATH = "datasets/lvis_1204.npy"
+SCANNET_CLASS_NAMES_PATH = "datasets/scannet_200_classname_no_wall_floor.npy"   # the text rows, in order
+SCANNET_CLASS_IDS_PATH = "datasets/scannet_200_class2id.npy"                     # {name: ScanNet-200 class id}
 
 
 class BoxProcessor(object):
@@ -88,16 +90,59 @@ class BoxProcessor(object):
         return self.dataset_config.box_parametrization_to_corners_xyz(box_center_unnorm, box_size_unnorm, box_angle)
 
 
+def _prompt(name) -> str:
+    return "a photo of a " + str(name).replace("_", " ").lower() + " in the scene"
+
+
+def scannet_class_rows(names, name_to_id) -> dict:
+    """ScanNet-200 class id -> its row in `names` (the class names without wall and floor), matched by name."""
+    row_of = {str(n): r for r, n in enumerate(names)}
+    return {int(i): row_of[str(n)] for n, i in name_to_id.items() if str(n) in row_of}
+
+
+def scannet_prompt_class_ids(train_ids, test_ids, reset_num: int) -> list:
+    """Class ids of the evaluated ScanNet prompts (reference :228-242): the seen classes, then the unseen classes of
+    `test_ids` in their order until `reset_num` of them have been added (at least one), sorted by id."""
+    ids, added = list(train_ids), 0
+    for c in test_ids:
+        if c in train_ids:
+            continue
+        ids.append(c)
+        added += 1
+        if added >= reset_num:
+            break
+    return sorted(ids)
+
+
+def _scannet_class_names(args):
+    if not (os.path.exists(SCANNET_CLASS_NAMES_PATH) and os.path.exists(SCANNET_CLASS_IDS_PATH)):
+        return None
+    names = np.load(SCANNET_CLASS_NAMES_PATH)
+    rows = scannet_class_rows(names, np.load(SCANNET_CLASS_IDS_PATH, allow_pickle=True).item())
+    train = [int(i) for i in args.train_range_list]
+    if getattr(args, "if_clip_more_prompts", False):
+        ids = scannet_prompt_class_ids(train, [int(i) for i in args.test_range_list], int(args.reset_scannet_num))
+    else:
+        ids = train                                  # the seen classes, in the order given
+    return [names[rows[i]] for i in ids]
+
+
 def _class_prompts(args):
     """'a photo of a {class} in the scene' prompts of the seen / evaluated classes
-    (reference :279).  Needs the class lists of a CoDA checkout (relative paths, as
-    in the reference); returns None when they are not reachable (synthetic runs)."""
+    (reference :197-279).  Needs the class lists of a CoDA checkout (relative paths, as
+    in the reference); returns None when they are not reachable (synthetic runs).
+    SUN RGB-D: the first train_range_max / test_range_max names of the class dictionary.
+    ScanNet (dataset_name contains "scannet"): the ScanNet-200 names picked by class id through
+    train_range_list / test_range_list / reset_scannet_num."""
+    if getattr(args, "dataset_name", "").find("scannet") != -1:
+        names = _scannet_class_names(args)
+        return None if names is None else [_prompt(c) for c in names]
     path = ALL_CLASS_PATH_V1 if getattr(args, "if_use_v1", True) else ALL_CLASS_PATH_V2
     if not os.path.exists(path):
         return None
     names = list(np.load(path, allow_pickle=True).item().keys())
     n = args.test_range_max if getattr(args, "if_clip_more_prompts", False) else args.train_range_max
-    return ["a photo of a " + c.replace("_", " ").lower() + " in the scene" for c in names[:n]]
+    return [_prompt(c) for c in names[:n]]
 
 
 class Model3DETRPredictedBoxDistillationHead(nn.Module):
@@ -373,8 +418,12 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
     def _boxes_in_image(self, inputs, outputs):
         """Every predicted box projected into the image: int32 (B, Q, 4) [xmin, ymin, xmax, ymax] (the reference's
         `int(torch.min/max(.))` truncation of non-negative fp64 values) and the boxes that are usable as crops
-        (non-degenerate, in front of the camera, non-zero size; reference :912-968, :1034-1051) -- one kernel."""
-        return ops.boxes_in_image(outputs["box_corners_xyz"].detach(), outputs["size_unnormalized"].detach(), inputs)
+        (non-degenerate, in front of the camera, non-zero size; reference :912-968, :1034-1051) -- one kernel, with
+        the dataset's camera model (reference :461-466)."""
+        # SUN RGB-D is the op's default camera: that call keeps its original form
+        camera = {"camera": "scannet"} if self.dataset_name == "scannet" else {}
+        return ops.boxes_in_image(outputs["box_corners_xyz"].detach(), outputs["size_unnormalized"].detach(), inputs,
+                                  **camera)
 
     @torch.no_grad()
     def _clip_embed_boxes(self, inputs, boxes, valid, sel, chosen=None):

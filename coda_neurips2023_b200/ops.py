@@ -712,32 +712,49 @@ def hungarian(cost: torch.Tensor, nactual: torch.Tensor):
     return inds, mask
 
 
+CAMERAS = {"sunrgbd": 0, "scannet": 1}      # include/coda_detr.h CODA_CAMERA_*; K / Rtilt are n x n per scene
+_CAMERA_DIM = {"sunrgbd": 3, "scannet": 4}
+
+
 @torch.no_grad()
-def boxes_in_image(corners_xyz: torch.Tensor, size_unnorm: torch.Tensor, inputs: dict):
+def boxes_in_image(corners_xyz: torch.Tensor, size_unnorm: torch.Tensor, inputs: dict, camera: str = "sunrgbd",
+                   extent: bool = False):
     """Predicted boxes (B, Q, 8, 3) -> (int32 (B, Q, 4) [xmin, ymin, xmax, ymax] in the image, bool (B, Q) usable as
-    a crop): include/coda_detr.h coda_boxes_in_image, fp64 like the reference's projection; no host sync."""
-    _need_cuda(corners_xyz, "boxes_in_image")
+    a crop): include/coda_detr.h coda_boxes_in_image, fp64 like the reference's projection; no host sync.
+    `camera` is the dataset's camera model: "sunrgbd" (K, Rtilt 3 x 3 intrinsics and tilt) or "scannet" (K the 4 x 4
+    colour intrinsics, Rtilt the 4 x 4 camera-to-world pose).  With `extent`, also the fp64 (B, Q, 4)
+    [umin, vmin, umax, vmax] the integer box truncates."""
+    if camera not in CAMERAS:
+        raise ValueError(f"boxes_in_image: unknown camera {camera!r} (expected one of {sorted(CAMERAS)})")
     b, q = corners_xyz.shape[:2]
+    n = _CAMERA_DIM[camera]
+    kshape, tshape = tuple(inputs["K"].shape), tuple(inputs["Rtilt"].shape)
+    if kshape != (b, n, n) or tshape != (b, n, n):
+        raise ValueError(f"boxes_in_image: the {camera} camera needs K and Rtilt of shape ({b}, {n}, {n}); "
+                         f"got K {kshape} and Rtilt {tshape}")
+    _need_cuda(corners_xyz, "boxes_in_image")
     dev = corners_xyz.device
     f64 = lambda t, shape: t.to(device=dev, dtype=torch.double).reshape(shape).contiguous()  # noqa: E731
     i64 = lambda t: t.to(device=dev, dtype=torch.int64).reshape(b).contiguous()  # noqa: E731
     scale = f64(inputs["scale_array"], (b, 3))
-    rot, K, Rtilt = f64(inputs["rot_array"], (b, 9)), f64(inputs["K"], (b, 9)), f64(inputs["Rtilt"], (b, 9))
+    rot, K, Rtilt = f64(inputs["rot_array"], (b, 9)), f64(inputs["K"], (b, n * n)), f64(inputs["Rtilt"], (b, n * n))
     flip, img_flip = f64(inputs["flip_array"], (b,)), f64(inputs["image_flip_array"], (b,))
     flip_len = f64(inputs["flip_length"], (b,))
     zx = f64(inputs["zx_flip_array"], (b,)) if "zx_flip_array" in inputs else None
     boxes = torch.empty((b, q, 4), dtype=torch.int32, device=dev)
     valid = torch.empty((b, q), dtype=torch.uint8, device=dev)
+    ext = torch.empty((b, q, 4), dtype=torch.double, device=dev) if extent else None
     # every converted operand is held in a local until the launch has been issued (a temporary that dies inside the
     # argument list would hand its block to the next conversion)
     cx, su = _f32c(corners_xyz), _f32c(size_unnorm)
     ow, oh, xo, yo = (i64(inputs[k]) for k in ("ori_width", "ori_height", "x_offset", "y_offset"))
     with torch.cuda.device(dev):
-        st = lib().coda_boxes_in_image(_i(b), _i(q), ptr(cx), ptr(su), ptr(scale), ptr(rot), ptr(flip), ptr(zx), ptr(K),
-                                       ptr(Rtilt), ptr(ow), ptr(oh), ptr(xo), ptr(yo), ptr(img_flip), ptr(flip_len),
-                                       ptr(boxes), ptr(valid), stream_of(corners_xyz))
+        st = lib().coda_boxes_in_image(_i(b), _i(q), _i(CAMERAS[camera]), ptr(cx), ptr(su), ptr(scale), ptr(rot),
+                                       ptr(flip), ptr(zx), ptr(K), ptr(Rtilt), ptr(ow), ptr(oh), ptr(xo), ptr(yo),
+                                       ptr(img_flip), ptr(flip_len), ptr(boxes), ptr(valid), ptr(ext),
+                                       stream_of(corners_xyz))
     check(st, "boxes_in_image")
-    return boxes, valid.bool()
+    return (boxes, valid.bool(), ext) if extent else (boxes, valid.bool())
 
 
 @torch.no_grad()

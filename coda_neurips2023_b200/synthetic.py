@@ -60,6 +60,19 @@ class SyntheticDatasetConfig:
         return get_3d_box_batch_tensor_xyz(box_size, box_angle, box_center_unnorm)
 
 
+SCANNET_TRAIN_RANGE_LIST = (2, 4, 5, 7, 13, 15, 16, 22, 56, 1163)
+SCANNET_TEST_RANGE_LIST = (
+    2, 4, 5, 6, 7, 8, 9, 10, 11, 13, 14, 15, 16, 17, 18, 19, 21, 22, 23, 24, 26, 27, 28, 29, 31, 32, 33, 34, 35, 36,
+    38, 39, 40, 41, 42, 44, 45, 46, 47, 48, 49, 50, 51, 52, 54, 55, 56, 57, 58, 59, 62, 63, 64, 65, 66, 67, 68, 69,
+    70, 71, 72, 73, 74, 75, 76, 77, 78, 79, 80, 82, 84, 86, 87, 88, 89, 90, 93, 95, 96, 97, 98, 99, 100, 101, 102,
+    103, 104, 105, 106, 107, 110, 112, 115, 116, 118, 120, 121, 122, 125, 128, 130, 131, 132, 134, 136, 138, 139,
+    140, 141, 145, 148, 154, 155, 156, 157, 159, 161, 163, 165, 166, 168, 169, 170, 177, 180, 185, 188, 191, 193,
+    195, 202, 208, 213, 214, 221, 229, 230, 232, 233, 242, 250, 261, 264, 276, 283, 286, 300, 304, 312, 323, 325,
+    331, 342, 356, 370, 392, 395, 399, 408, 417, 488, 540, 562, 570, 572, 581, 609, 748, 776, 1156, 1163, 1164,
+    1165, 1166, 1167, 1168, 1169, 1170, 1171, 1172, 1173, 1174, 1175, 1176, 1178, 1179, 1180, 1181, 1182, 1183,
+    1184, 1185, 1186, 1187, 1188, 1189, 1190, 1191)
+
+
 def make_args(**overrides) -> argparse.Namespace:
     """Defaults of the reference's main.py argument parser (main.py:37-304) for every field
     the model / criterion read, overlaid with scripts/coda_sunrgbd_stage1.sh, overlaid with
@@ -85,6 +98,10 @@ def make_args(**overrides) -> argparse.Namespace:
         base_lr=1.97e-4, warm_lr=1e-6, warm_lr_epochs=18, final_lr=1e-6, lr_scheduler="cosine",
         weight_decay=0.1, filter_biases_wd=False, clip_gradient=0.1, max_epoch=1080,
         batchsize_per_gpu=8, ngpus=1,
+        # ScanNet-200 class ids of the seen / evaluated prompts and the cap on added unseen classes (main.py:245-247;
+        # scripts/coda_scannet_stage1.sh); read only when dataset_name names ScanNet
+        train_range_list=list(SCANNET_TRAIN_RANGE_LIST), test_range_list=list(SCANNET_TEST_RANGE_LIST),
+        reset_scannet_num=50,
     )
     a.update(overrides)
     return argparse.Namespace(**a)
@@ -104,10 +121,15 @@ def _corners_np(size, angle, center_cam):
 
 
 def make_batch(batch: int, npoints: int = 20000, seed: int = 0, max_gt: int = 64, image_hw=(531, 730),
-               num_angle_bin: int = 12, ncls_seen: int = 10, min_gt: int = 3, max_real_gt: int = 20):
+               num_angle_bin: int = 12, ncls_seen: int = 10, min_gt: int = 3, max_real_gt: int = 20,
+               camera: str = "sunrgbd"):
     """One SUN RGB-D-shaped training batch as numpy arrays / what the dataloader collates
     (datasets/sunrgbd_anonymous_aligned_image.py:813-899; SURVEY.md section 8d).  fp64 where
-    the reference's numpy arrays are fp64 (K, Rtilt, rot_array, scale_array, flip arrays)."""
+    the reference's numpy arrays are fp64 (K, Rtilt, rot_array, scale_array, flip arrays).
+    camera="scannet": the image side of a ScanNet batch instead (datasets/scannet_anonymous_aligned_image.py:537-702,
+    see _scannet_camera); the point cloud and the boxes are drawn the same way."""
+    if camera not in ("sunrgbd", "scannet"):
+        raise ValueError(f"unknown camera {camera!r}")
     rng = np.random.default_rng(seed + 7919)
     pc = point_clouds(batch, npoints, seed=seed)
     h, w = image_hw
@@ -146,6 +168,10 @@ def make_batch(batch: int, npoints: int = 20000, seed: int = 0, max_gt: int = 64
         "gt_box_seen_sem_cls_label": rng.integers(0, ncls_seen, size=(batch, max_gt)).astype(np.int64),
         "gt_box_seen_sem_cls_confi": present.copy(),
     })
+    if camera == "scannet":
+        d.update(_scannet_camera(rng, batch, h, w))
+        d["gt_ori_box_num"] = present.sum(axis=1).astype(np.int64)
+        return d
     # image side: SUN RGB-D-like intrinsics, small tilt, augmentation bookkeeping
     # SUN RGB-D intrinsics at 730 x 531; other image shapes (ScanNet: 1296 x 968) scale the focal length with
     # the width and keep the principal point at the same relative position
@@ -169,6 +195,67 @@ def make_batch(batch: int, npoints: int = 20000, seed: int = 0, max_gt: int = 64
         "gt_ori_box_num": present.sum(axis=1).astype(np.int64),
     })
     return d
+
+
+def rotz(t: float) -> np.ndarray:
+    c, s = np.cos(t), np.sin(t)
+    return np.array([[c, -s, 0.0], [s, c, 0.0], [0.0, 0.0, 1.0]])
+
+
+# ScanNet colour-camera intrinsics (intrinsic/intrinsic_color.txt of a typical scene, 1296 x 968)
+SCANNET_COLOR_FOCAL = 1170.19
+SCANNET_COLOR_CENTER = (647.75, 483.75)
+SCANNET_CAMERA_DISTANCE = (-1.2, -0.8)     # along the heading of the room's centre from the origin, m
+
+
+def _scannet_camera(rng, batch: int, h: int, w: int) -> dict:
+    """Image side of a ScanNet batch (datasets/scannet_anonymous_aligned_image.py:537-702): K the 4 x 4 colour
+    intrinsics scaled to the image size, Rtilt the 4 x 4 camera-to-world pose, and ScanNet's augmentation
+    bookkeeping (x flip, zx flip, rotation within +-30 degrees with rot_array = inv(rotz^T), scale).
+
+    The pose lives in the scene's frame before augmentation, where the flips and the rotation put the synthetic
+    room anywhere around the origin.  The camera stands 1.5 m above the room's floor, 0.8 .. 1.2 m behind the origin
+    as seen from the room's centre, and looks towards the centre with a small yaw and a downward pitch; the camera
+    frame is x right, y down, z forward, as in ScanNet.  With the metre-sized boxes of an untrained model this
+    gives, in every scene, boxes inside the image, boxes clipped at an image edge and boxes behind the camera."""
+    rot = rng.uniform(-np.pi / 6, np.pi / 6, size=batch)
+    rot_array = np.stack([np.linalg.inv(rotz(t).T) for t in rot])
+    flip = rng.choice([-1.0, 1.0], size=(batch, 1)).astype(np.float64)
+    zx_flip = rng.choice([-1.0, 1.0], size=(batch, 1)).astype(np.float64)
+    scale = rng.uniform(0.9, 1.1, size=(batch, 1, 1)).repeat(3, axis=2).astype(np.float64)
+    image_flip = rng.choice([0.0, 1.0], size=(batch, 1)).astype(np.float64)
+    yaw = rng.uniform(-np.pi / 12, np.pi / 12, size=batch)
+    pitch = rng.uniform(np.pi / 36, np.pi / 9, size=batch)               # 5 .. 20 degrees down
+    dist = rng.uniform(*SCANNET_CAMERA_DISTANCE, size=batch)
+    height = rng.uniform(-0.1, 0.1, size=batch)
+    sx, sy = w / 1296.0, h / 968.0
+    K = np.zeros((batch, 4, 4))
+    K[:, 0, 0], K[:, 1, 1] = SCANNET_COLOR_FOCAL * sx, SCANNET_COLOR_FOCAL * sy
+    K[:, 0, 2], K[:, 1, 2] = SCANNET_COLOR_CENTER[0] * sx, SCANNET_COLOR_CENTER[1] * sy
+    K[:, 2, 2] = K[:, 3, 3] = 1.0
+    pose = np.zeros((batch, 4, 4))
+    for b in range(batch):
+        centre = (0.5 * (ROOM_MIN + ROOM_MAX)).astype(np.float64) * scale[b, 0] @ rot_array[b]   # augmentation undone
+        centre[1] *= zx_flip[b, 0]
+        centre[0] *= flip[b, 0]
+        head = np.arctan2(centre[0], centre[1])                           # heading of the centre, from +y towards +x
+        fwd = np.array([np.sin(head + yaw[b]) * np.cos(pitch[b]), np.cos(head + yaw[b]) * np.cos(pitch[b]),
+                        -np.sin(pitch[b])])
+        right = np.array([np.cos(head + yaw[b]), -np.sin(head + yaw[b]), 0.0])
+        pose[b, :3, :3] = np.stack((right, np.cross(fwd, right), fwd), axis=1)   # columns: camera axes in the world
+        pose[b, :3, 3] = (dist[b] * np.sin(head), dist[b] * np.cos(head), ROOM_MIN[2] + 1.5 + height[b])
+        pose[b, 3, 3] = 1.0
+    # a pose read from text is not exactly orthonormal: keep it as printed with 6 decimals
+    pose = np.round(pose, 6)
+    return {
+        "input_image": rng.integers(0, 256, size=(batch, h, w, 3), dtype=np.uint8),
+        "K": K, "Rtilt": pose, "rot_array": rot_array, "flip_array": flip, "zx_flip_array": zx_flip,
+        "scale_array": scale, "image_flip_array": image_flip,
+        "flip_length": np.full((batch,), float(w), np.float64),
+        "ori_width": np.full((batch,), w, np.int64), "ori_height": np.full((batch,), h, np.int64),
+        "x_offset": np.zeros((batch,), np.int64), "y_offset": np.zeros((batch,), np.int64),
+        "rot_angle": rot.astype(np.float64),
+    }
 
 
 def to_device(batch_np: dict, device, pinned: bool = False) -> dict:

@@ -147,19 +147,28 @@ int coda_novel_candidates(int b, int q, int g, int cap, const int *boxes2d, cons
 
 /*
  * Predicted 3-D boxes -> integer 2-D boxes in the image + usability flags, one thread per box, fp64.
- *   replaces models/model_3detr.py:912-968 (undo scale / rotation / flips of the point-cloud augmentation),
- *   datasets/sunrgbd_utils.py:611-635 (project_3dpoint_to_2dpoint_corners_tensor), the clipping / offset / image-flip
- *   bookkeeping (:950-968) and the per-box checks (:1034-1051).
- *   corners_xyz (b, q, 8, 3) fp32, size_unnorm (b, q, 3) fp32; per scene (fp64): scale (3), rot (3x3, applied as
- *   p @ rot), flip, zx_flip (NULL = absent), K (3x3), Rtilt (3x3), img_flip, flip_len; (int64): ori_w, ori_h, x_off,
+ *   replaces models/model_3detr.py:912-968 (undo scale / rotation / flips of the point-cloud augmentation), the
+ *   dataset's project_3dpoint_to_2dpoint_corners_tensor, the clipping / offset / image-flip bookkeeping (:950-968)
+ *   and the per-box checks (:1034-1051).  `camera` picks the dataset's camera model (model_3detr.py:461-466):
+ *     CODA_CAMERA_SUNRGBD  datasets/sunrgbd_utils.py:611-635: K (3x3 intrinsics), Rtilt (3x3 tilt);
+ *                          p_cam = axis swap of Rtilt^T p, uv = K p_cam.
+ *     CODA_CAMERA_SCANNET  datasets/scannet_utils.py:650-690: K (4x4 intrinsic_color), Rtilt (4x4 camera-to-world
+ *                          pose); p_cam = inv(pose) [p, 1] (rows 0..2; the inverse by Gauss-Jordan with partial
+ *                          pivoting, once per scene, fp64), uv = K[:3, :3] p_cam.
+ *   Both: pixel = uv[0:2] / (uv[2] + 1e-32), depth = uv[2].
+ *   corners_xyz (b, q, 8, 3) fp32, size_unnorm (b, q, 3) fp32; per scene (fp64, row-major): scale (3), rot (3x3,
+ *   applied as p @ rot), flip, zx_flip (NULL = absent), K, Rtilt, img_flip, flip_len; (int64): ori_w, ori_h, x_off,
  *   y_off.  boxes (b, q, 4) int32 [xmin, ymin, xmax, ymax] (truncation, like int(torch.min(.)));
- *   valid (b, q) uint8 = (xmax > xmin) & (ymax > ymin) & (min depth >= 0) & !(max size < 1e-16).
+ *   valid (b, q) uint8 = (xmax > xmin) & (ymax > ymin) & (min depth >= 0) & !(max size < 1e-16) (and, ScanNet, a
+ *   non-singular pose); extent (b, q, 4) fp64 [umin, vmin, umax, vmax] before truncation, or NULL (not written).
  */
-int coda_boxes_in_image(int b, int q, const float *corners_xyz, const float *size_unnorm, const double *scale,
-                        const double *rot, const double *flip, const double *zx_flip, const double *K,
-                        const double *Rtilt, const long long *ori_w, const long long *ori_h, const long long *x_off,
-                        const long long *y_off, const double *img_flip, const double *flip_len, int *boxes,
-                        unsigned char *valid, void *stream);
+#define CODA_CAMERA_SUNRGBD 0
+#define CODA_CAMERA_SCANNET 1
+int coda_boxes_in_image(int b, int q, int camera, const float *corners_xyz, const float *size_unnorm,
+                        const double *scale, const double *rot, const double *flip, const double *zx_flip,
+                        const double *K, const double *Rtilt, const long long *ori_w, const long long *ori_h,
+                        const long long *x_off, const long long *y_off, const double *img_flip,
+                        const double *flip_len, int *boxes, unsigned char *valid, double *extent, void *stream);
 
 #ifdef __cplusplus
 }
