@@ -122,16 +122,20 @@ def forward(q, k, v, nhead: int, dropout_p: float = 0.0, salt: int = 0, nsplit: 
 
 
 def forward_half(q, k, v, nhead: int):
-    """fp16 q / k / v (L <= 64, B, H * 64), contiguous or row-strided slices of a fused projection -> fp16 (L, B, E):
-    the CLIP image tower's attention on half operands (include/coda_attention.h coda_attention_fwd_half)."""
+    """fp16 q / k / v (L <= 256, B, H * 64), contiguous or row-strided slices of a fused projection -> fp16 (L, B, E):
+    the CLIP image tower's attention on half operands (include/coda_attention.h coda_attention_fwd_half).  Above 64
+    tokens (ViT-B/16) the kernel reads q / k / v in place by TMA and needs no workspace."""
     l, b, e = q.shape
-    assert q.dtype == k.dtype == v.dtype == torch.float16 and e // nhead == 64 and l <= 64 and k.shape[0] == l
+    assert q.dtype == k.dtype == v.dtype == torch.float16 and e // nhead == 64 and l <= 256 and k.shape[0] == l
     lds = [_row_strided(t) for t in (q, k, v)]
+    if l > 64:   # TMA reads the slices in place: 16-byte aligned bases and row strides
+        lds = [ld if ld is not None and ld % 8 == 0 and t.data_ptr() % 16 == 0 else None
+               for ld, t in zip(lds, (q, k, v))]
     if any(ld is None for ld in lds):
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
         lds = [e, e, e]
     out = torch.empty((l, b, e), dtype=torch.float16, device=q.device)
-    ws = torch.empty(3 * b * nhead * l * 64 * 2 + 512, dtype=torch.uint8, device=q.device)
+    ws = None if l > 64 else torch.empty(3 * b * nhead * l * 64 * 2 + 512, dtype=torch.uint8, device=q.device)
     cl = ctypes.c_longlong
     with torch.cuda.device(q.device):
         st = lib().coda_attention_fwd_half(ctypes.c_int(b), ctypes.c_int(nhead), ctypes.c_int(l), ctypes.c_int(64), ptr(q),

@@ -70,9 +70,10 @@ class _PackedSelfAttention(nn.Module):
         q, k, v = _linear(x, self.in_proj_weight, self.in_proj_bias).split(self.embed_dim, dim=-1)
         if x.is_cuda and x.dtype == torch.float16 and not causal and self.embed_dim // self.num_heads == 64:
             from .. import attention_launch
-            # q / k / v stay fp16 slices of the fused projection: the pack kernel reads them in place
-            if x.shape[0] <= 64:
-                # image tower (50 tokens): fused wgmma attention on HALF operands, the tensor core's native type
+            # q / k / v stay fp16 slices of the fused projection: the attention kernels read them in place
+            if x.shape[0] <= 256:
+                # image tower (ViT-B/32: 50 tokens, ViT-B/16: 197): fused wgmma attention on HALF operands, the
+                # tensor core's native type
                 out = attention_launch.forward_half(q, k, v, self.num_heads)
             else:
                 # longer sequences: 2 bf16 planes (16 mantissa bits >= fp16's 11)

@@ -356,6 +356,165 @@ int launch_attn(const AttnMaps &maps, int Lq, int Lk, int B, int H, float *out, 
   return launch_status();
 }
 
+// ------------------------------------------------------------------ fp16 self-attention, 64 < L <= 256, hd 64
+// The CLIP ViT-B/16 image tower (197 tokens).  One CTA per (crop, head): every Q, K and V tile of the sequence is
+// loaded ONCE by TMA straight out of the fused in-projection output (L, N, ld) -- no pack pass, no workspace -- and
+// stays resident in shared memory; the query tiles are spread over the warpgroups, and each walks all key tiles with
+// the online softmax of attn_fwd_kernel.  The maps are 3-D: the head and head-dim indices are contiguous, so
+// (h * 64 + d, token, crop) addresses q / k / v with a token stride of N * ld; TMA zero-fills tokens >= L.
+struct HalfMaps {
+  CUtensorMap q, k, v;
+};
+
+struct ResCfg {
+  static constexpr int NT = 4;                  // tiles of 64 tokens: L <= 256
+  static constexpr int NWG = 2;                 // warpgroups; warpgroup w takes query tiles w and w + 2
+  static constexpr int BOX = 64 * 128;          // one [64 tokens x 64] half box
+  static constexpr int Q_OFF = 0, K_OFF = NT * BOX, V_OFF = 2 * NT * BOX;
+  static constexpr int TOTAL = 3 * NT * BOX;    // 96 KB: two CTAs per SM
+  static constexpr int THREADS = NWG * 128;
+};
+
+// qk_scale = log2(e) / sqrt(hd), applied to the fp32 scores: the softmax works in base 2 (one ex2 per element)
+__global__ void __launch_bounds__(ResCfg::THREADS, 2)
+attn_fwd_half_resident_kernel(const __grid_constant__ HalfMaps maps, int L, int B, int H, float qk_scale,
+                              __half *__restrict__ out) {
+  using C = ResCfg;
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  unsigned char *smem = smem_align1024(smem_raw);
+  __shared__ __align__(8) uint64_t q_full[C::NT], kv_full[C::NT];   // each completes once: phase parity 0
+
+  const int bh = blockIdx.x, b = bh / H, h = bh - b * H;
+  const int nt = (L + 63) / 64;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < C::NT; ++i) { mbar_init(&q_full[i], 1); mbar_init(&kv_full[i], 1); }
+    mbar_fence_init_cluster();
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    // the first query tile of each warpgroup, then K_j / V_j in the order they are walked, then the second round
+    auto load_q = [&](int t) {
+      mbar_arrive_expect_tx(&q_full[t], (uint32_t)C::BOX);
+      tma_load_3d(smem + C::Q_OFF + t * C::BOX, &maps.q, &q_full[t], h * 64, t * 64, b);
+    };
+    for (int t = 0; t < C::NWG && t < nt; ++t) load_q(t);
+    for (int j = 0; j < nt; ++j) {
+      mbar_arrive_expect_tx(&kv_full[j], (uint32_t)(2 * C::BOX));
+      tma_load_3d(smem + C::K_OFF + j * C::BOX, &maps.k, &kv_full[j], h * 64, j * 64, b);
+      tma_load_3d(smem + C::V_OFF + j * C::BOX, &maps.v, &kv_full[j], h * 64, j * 64, b);
+    }
+    for (int t = C::NWG; t < nt; ++t) load_q(t);
+  }
+
+  // thread rows r0 = 16 wl + g and r0 + 8 of the warpgroup's 64, columns 8 c + 2 t4 + {0, 1}
+  const int w = threadIdx.x >> 7, wl = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, g = lane >> 2, t4 = lane & 3;
+  for (int t = w; t < nt; t += C::NWG) {
+    const int qrow[2] = {t * 64 + wl * 16 + g, t * 64 + wl * 16 + g + 8};
+    float o_acc[32];
+    acc_zero(o_acc);
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // m_run: raw score units
+    const unsigned char *qs = smem + C::Q_OFF + t * C::BOX;
+    mbar_wait(&q_full[t], 0);
+    for (int j = 0; j < nt; ++j) {
+      const unsigned char *ks = smem + C::K_OFF + j * C::BOX, *vs = smem + C::V_OFF + j * C::BOX;
+      mbar_wait(&kv_full[j], 0);
+      float sacc[32];
+      acc_fence(sacc);
+      wgmma_fence();
+      const uint64_t ad = gmma_desc_k_sw128(qs), bd = gmma_desc_k_sw128(ks);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+        Wgmma<KT, true>::ss<0, 0>(sacc, gmma_desc_advance(ad, kk * 32), gmma_desc_advance(bd, kk * 32), kk != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(sacc);
+
+      const int kvalid = L - j * KT;  // keys >= kvalid are TMA's zero fill (last tile only)
+      float alpha[2], mc[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float mloc = -INFINITY;
+#pragma unroll
+        for (int c = 0; c < KT / 8; ++c)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float &x = sacc[c * 4 + i * 2 + e];
+            if (c * 8 + 2 * t4 + e >= kvalid) x = -INFINITY;
+            mloc = fmaxf(mloc, x);
+          }
+        mloc = fmaxf(mloc, __shfl_xor_sync(0xffffffffu, mloc, 1));
+        mloc = fmaxf(mloc, __shfl_xor_sync(0xffffffffu, mloc, 2));
+        // tile 0 always holds a valid key (L > 0), so the running max is finite from the first tile on
+        const float m_new = fmaxf(m_run[i], mloc);
+        alpha[i] = ex2_approx((m_run[i] - m_new) * qk_scale);   // -inf on the first tile -> 0
+        mc[i] = m_new * qk_scale;
+        m_run[i] = m_new;
+      }
+      // P_j = 2^(s * qk_scale - m * qk_scale) -> fp16 A fragments (key chunk c of 8: k-step c / 2, register
+      // (c & 1) * 2 + i)
+      uint32_t pf[KT / 16][4];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float lsum = 0.f;
+#pragma unroll
+        for (int c = 0; c < KT / 8; ++c) {
+          const float r0 = ex2_approx(fmaf(sacc[c * 4 + i * 2], qk_scale, -mc[i]));
+          const float r1 = ex2_approx(fmaf(sacc[c * 4 + i * 2 + 1], qk_scale, -mc[i]));
+          lsum += r0 + r1;
+          pf[c >> 1][(c & 1) * 2 + i] = pack2<true>(r0, r1);
+        }
+        l_run[i] = l_run[i] * alpha[i] + lsum;
+      }
+      // o = o * alpha + P_j V_j: rescale the running accumulator in place, then accumulate into it
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        o_acc[c * 4] *= alpha[0];
+        o_acc[c * 4 + 1] *= alpha[0];
+        o_acc[c * 4 + 2] *= alpha[1];
+        o_acc[c * 4 + 3] *= alpha[1];
+      }
+      acc_fence(o_acc);
+      wgmma_fence();
+      const uint64_t vd = gmma_desc_mn_sw128(vs);
+#pragma unroll
+      for (int kk = 0; kk < KT / 16; ++kk) Wgmma<64, true>::rs<1>(o_acc, pf[kk], gmma_desc_advance(vd, kk * 16 * 128), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(o_acc);
+    }
+    // normalise and store rows < L of (L, B, H * 64) as half
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float l = l_run[i];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      if (qrow[i] >= L) continue;
+      const float inv = 1.0f / l;
+      __half *orow = out + ((size_t)qrow[i] * B + b) * (size_t)(H * 64) + (size_t)h * 64;
+#pragma unroll
+      for (int c = 0; c < 8; ++c)
+        *reinterpret_cast<__half2 *>(orow + c * 8 + 2 * t4) =
+            __floats2half2_rn(o_acc[c * 4 + i * 2] * inv, o_acc[c * 4 + i * 2 + 1] * inv);
+    }
+  }
+}
+
+// q / k / v: (l, b, ld) half with the h * 64 head columns at the front of each row
+int launch_attn_half_resident(int b, int h, int l, const void *q, const void *k, const void *v, long long ld_q,
+                              long long ld_k, long long ld_v, __half *out, cudaStream_t s) {
+  HalfMaps maps;
+  const long long e = (long long)h * 64;
+  int st = make_tmap_k_major_16b(&maps.q, q, 1, e, l, b, (long long)b * ld_q, ld_q, 64);
+  if (st == CODA_OK) st = make_tmap_k_major_16b(&maps.k, k, 1, e, l, b, (long long)b * ld_k, ld_k, 64);
+  if (st == CODA_OK) st = make_tmap_k_major_16b(&maps.v, v, 1, e, l, b, (long long)b * ld_v, ld_v, 64);
+  if (st != CODA_OK) return st;
+  constexpr auto kern = attn_fwd_half_resident_kernel;
+  const int smem = ResCfg::TOTAL + 1024;
+  if (const int r = raise_smem_limit<kern>(smem)) return r;
+  kern<<<b * h, ResCfg::THREADS, smem, s>>>(maps, l, b, h, LOG2E / sqrtf(64.f), out);
+  return launch_status();
+}
+
 }  // namespace
 
 extern "C" {
@@ -459,11 +618,20 @@ int coda_attention_fwd_packed_masked(int b, int h, int lq, int lk, int hd, int n
 
 int coda_attention_fwd_half(int b, int h, int l, int hd, const void *q, const void *k, const void *v, long long ld_q,
                             long long ld_k, long long ld_v, void *out, void *workspace, void *stream) {
-  // fp16 self-attention of at most one key tile (the CLIP image tower: 50 tokens, 12 x 64): q / k / v are read as
-  // half (row-strided slices of the fused projection), re-laid as ONE plane of half operands -- fp16 is the tensor
-  // core's native type, no bf16 split -- and the output is written as half.
-  if (b < 0 || h <= 0 || l <= 0 || l > KT || hd != 64 || (long long)b * h > 65535) return CODA_EINVAL;
+  // fp16 self-attention (the CLIP image tower, 12 x 64 heads).  At most one key tile (ViT-B/32: 50 tokens): q / k / v
+  // are read as half (row-strided slices of the fused projection), re-laid as ONE plane of half operands -- fp16 is
+  // the tensor core's native type, no bf16 split -- and the output is written as half.  Up to four key tiles
+  // (ViT-B/16: 197 tokens): the resident kernel reads q / k / v by TMA in place, without a workspace.
+  if (b < 0 || h <= 0 || l <= 0 || l > ResCfg::NT * KT || hd != 64 || (long long)b * h > 65535) return CODA_EINVAL;
   if (b == 0) return CODA_OK;
+  if (l > KT) {
+    if (!q || !k || !v || !out) return CODA_EINVAL;
+    // TMA: 16-byte aligned bases and row strides
+    if ((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) != 0 || ((ld_q | ld_k | ld_v) & 7) != 0) return CODA_EINVAL;
+    if (ld_q < (long long)h * hd || ld_k < (long long)h * hd || ld_v < (long long)h * hd) return CODA_EINVAL;
+    return launch_attn_half_resident(b, h, l, q, k, v, ld_q, ld_k, ld_v, reinterpret_cast<__half *>(out),
+                                     (cudaStream_t)stream);
+  }
   if (!q || !k || !v || !out || !workspace) return CODA_EINVAL;
   if ((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 7) != 0 || ((ld_q | ld_k | ld_v) & 3) != 0) return CODA_EINVAL;
   if (ld_q < (long long)h * hd || ld_k < (long long)h * hd || ld_v < (long long)h * hd) return CODA_EINVAL;

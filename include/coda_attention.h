@@ -59,10 +59,15 @@ int coda_attention_fwd_packed_ex(int b, int h, int lq, int lk, int hd, int nspli
                                  const unsigned int *seed_dev, void *stream);
 
 /*
- * fp16 self-attention with at most 64 tokens and head dim 64 (the CLIP ViT image tower, CLIP/clip/model.py:295-316 --
- * nn.MultiheadAttention on fp16 activations): q, k, v (l, b, h*64) IEEE half with row strides ld_* (slices of the fused
- * in-projection), out (l, b, h*64) half.  Operands stay half: one plane, one wgmma per product.
- * workspace: 3 * b*h*l*64 halves + 256 bytes.
+ * fp16 self-attention with at most 256 tokens and head dim 64, no mask, no dropout (the CLIP ViT image tower,
+ * CLIP/clip/model.py:295-316 -- nn.MultiheadAttention on fp16 activations; ViT-B/32: 50 tokens, ViT-B/16: 197):
+ * q, k, v (l, b, h*64) IEEE half with row strides ld_* (slices of the fused in-projection), out (l, b, h*64) half,
+ * contiguous.  Operands stay half: one plane, one wgmma per product.
+ *   l <= 64: q / k / v are re-laid into `workspace` (3 * b*h*l*64 halves + 256 bytes) with q pre-scaled, then one
+ *     key tile is attended.  ld_* multiples of 4, bases 8-byte aligned.
+ *   64 < l <= 256: one kernel reads q / k / v in place by TMA and applies the scale to the fp32 scores; `workspace`
+ *     is not used and may be NULL.  ld_* multiples of 8, bases 16-byte aligned.
+ * l > 256, hd != 64 or a base / row stride outside these rules: CODA_EINVAL.
  */
 int coda_attention_fwd_half(int b, int h, int l, int hd, const void *q, const void *k, const void *v, long long ld_q,
                             long long ld_k, long long ld_v, void *out, void *workspace, void *stream);
