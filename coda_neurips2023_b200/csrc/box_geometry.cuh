@@ -21,14 +21,22 @@ __device__ __forceinline__ P2 sh_intersect(P2 cp1, P2 cp2, P2 s, P2 e) {
 
 // Sutherland-Hodgman clip of quadrilateral `subj` by convex quadrilateral `clip`
 // (utils/box_util.py:540-578); returns twice-unsigned-area / 2 of the result.
+// The area does not depend on where the pair stands, but sh_intersect and the shoelace sum multiply coordinates and
+// subtract the products, so their rounding error grows with |coordinate|^2: all eight points are first taken relative
+// to clip[0] (differences of nearby fp32 numbers, exact or correctly rounded at the scale of the pair), which keeps
+// the error a property of the two boxes wherever in the scene they are.
 __device__ inline float clipped_area(const P2 *subj, const P2 *clip) {
-  P2 a[10], bq[10];
+  P2 a[10], bq[10], cl[4];
   int na = 4;
+  const P2 org = clip[0];
 #pragma unroll
-  for (int i = 0; i < 4; ++i) a[i] = subj[i];
-  P2 cp1 = clip[3];
+  for (int i = 0; i < 4; ++i) {
+    a[i] = P2{subj[i].x - org.x, subj[i].y - org.y};
+    cl[i] = P2{clip[i].x - org.x, clip[i].y - org.y};
+  }
+  P2 cp1 = cl[3];
   for (int ci = 0; ci < 4; ++ci) {
-    const P2 cp2 = clip[ci];
+    const P2 cp2 = cl[ci];
     int nb = 0;
     P2 s = a[na - 1];
     for (int i = 0; i < na; ++i) {

@@ -51,6 +51,9 @@ points_in_boxes_kernel(int k, int n, int pstride, const float *__restrict__ corn
   }
   // inclusive faces, with the slack a hull test in double precision has around an fp32 box
   const float eu = 1e-6f * uu, ev = 1e-6f * vv, ew = 1e-6f * ww;
+  // a box with an edge of length zero (the all-zero padding box among them) has no inside: without this every
+  // comparison below reads 0 >= -0 && 0 <= 0 along that edge and the flat box would collect the points of its plane
+  const bool solid = live && uu > 0.f && vv > 0.f && ww > 0.f;
   int cnt = 0;
   for (int p0 = 0; p0 < n; p0 += PIB_TILE) {
     const int m = min(PIB_TILE, n - p0);
@@ -60,7 +63,7 @@ points_in_boxes_kernel(int k, int n, int pstride, const float *__restrict__ corn
       pts[i] = make_float3(p[0], p[1], p[2]);
     }
     __syncthreads();
-    if (live) {
+    if (solid) {
       for (int i = 0; i < m; ++i) {
         const float dx = pts[i].x - o.x, dy = pts[i].y - o.y, dz = pts[i].z - o.z;
         const float a = dx * u.x + dy * u.y + dz * u.z;
@@ -75,8 +78,9 @@ points_in_boxes_kernel(int k, int n, int pstride, const float *__restrict__ corn
 
 // ------------------------------------------------------------------ 3-D NMS
 // One CTA per scene.  Boxes enter by their axis-aligned extents in the frame they are given in (the reference feeds
-// the camera-frame corners, ap_calculator.py:877-899); candidates = valid boxes; greedy from the highest score
-// (utils/nms.py:90-116 walks np.argsort(score) from the back: among equal scores the higher index goes first).
+// the camera-frame corners, ap_calculator.py:877-899); candidates = valid boxes whose score is not NaN; greedy from
+// the highest score (utils/nms.py:90-116 walks np.argsort(score) from the back: among equal scores the higher index
+// goes first).
 constexpr int NMS_MAXK = 2048;
 
 __global__ void __launch_bounds__(256)
@@ -103,24 +107,29 @@ nms3d_kernel(int k, const float *__restrict__ corners, const float *__restrict__
     lo[3 * i] = l0; lo[3 * i + 1] = l1; lo[3 * i + 2] = l2;
     hi[3 * i] = h0; hi[3 * i + 1] = h1; hi[3 * i + 2] = h2;
     vol[i] = (h0 - l0) * (h1 - l1) * (h2 - l2);
-    const bool ok = valid[(size_t)b * k + i] != 0;
-    sc[i] = ok ? score[(size_t)b * k + i] : -INFINITY;
+    const float s = score[(size_t)b * k + i];
+    const bool ok = valid[(size_t)b * k + i] != 0 && s == s;   // a NaN score cannot be ranked: not a candidate
+    sc[i] = ok ? s : -INFINITY;
     kl[i] = cls ? cls[(size_t)b * k + i] : 0;
     dead[i] = ok ? 0 : 1;
     keep[(size_t)b * k + i] = 0;
   }
   if (tid == 0) ncand = 0;
   __syncthreads();
-  // rank by counting: descending score, ties -> higher index first; non-candidates sink to the end
+  // rank by counting on the pair (candidate?, score): candidates first, by descending score, ties -> higher index
+  // first; then the non-candidates by index.  Candidate scores are never NaN, so this is a total order and order[]
+  // a permutation of 0..k-1 whose first ncand entries are the candidates (a candidate scored -inf included).
   for (int i = tid; i < k; i += blockDim.x) {
     const float s = sc[i];
+    const bool ci = !dead[i];
     int r = 0;
     for (int j = 0; j < k; ++j) {
       const float t = sc[j];
-      r += (t > s) || (t == s && j > i);
+      const bool cj = !dead[j];
+      r += (cj != ci) ? cj : (ci ? ((t > s) || (t == s && j > i)) : (j > i));
     }
     order[r] = i;
-    if (!dead[i]) atomicAdd(&ncand, 1);
+    if (ci) atomicAdd(&ncand, 1);
   }
   __syncthreads();
   const int nc = ncand;

@@ -20,7 +20,9 @@ extern "C" {
  *   replaces the `remove_empty_box` loop of parse_predictions (utils/ap_calculator.py:808-835): per box
  *   flip_axis_to_depth + extract_pc_in_box3d (utils/box_util.py:22-31, a scipy Delaunay hull test on the host).
  *   corners_camera (b, k, 8, 3) camera frame; points_depth (b, n, point_stride) fp32 in the upright DEPTH frame
- *   (depth (X, Y, Z) = camera (X, Z, -Y)), only the first three columns are read.  An all-zero box counts 0.
+ *   (depth (X, Y, Z) = camera (X, Z, -Y)), only the first three columns are read.  Faces are inclusive: a point on
+ *   a face, an edge or a corner of the box is inside.  A box with an edge of length zero -- the all-zero box, a box
+ *   of zero height -- has no inside and counts 0.
  */
 int coda_points_in_boxes(int b, int k, int n, int point_stride, const float *corners_camera, const float *points_depth,
                          int *counts, void *stream);
@@ -28,9 +30,11 @@ int coda_points_in_boxes(int b, int k, int n, int point_stride, const float *cor
 /*
  * Greedy 3-D non-maximum suppression per scene on the axis-aligned extents of the corners.
  *   replaces nms_3d_faster / nms_3d_faster_samecls (utils/nms.py:79-162) and the per-scene Python loops that build
- *   their input (utils/ap_calculator.py:868-941).  Candidates are the boxes with valid != 0; visited from the
- *   highest score; a later box is dropped when inter / (vol_i + vol_j - inter) > iou_thresh (old_type: inter / vol_j)
- *   and -- if cls is not NULL -- it has the same class.  keep (b, k) uint8, k <= 2048.
+ *   their input (utils/ap_calculator.py:868-941).  Candidates are the boxes with valid != 0 whose score is not NaN
+ *   (a NaN cannot be ranked; such a box is never kept, whatever `valid` says; -inf and +inf are ordinary scores);
+ *   visited from the highest score, among equal scores the higher index first; a later box is dropped when
+ *   inter / (vol_i + vol_j - inter) > iou_thresh (old_type: inter / vol_j) and -- if cls is not NULL -- it has the
+ *   same class.  keep (b, k) uint8, k <= 2048.
  */
 int coda_nms3d(int b, int k, const float *corners, const float *score, const int *cls, const unsigned char *valid,
                float iou_thresh, int old_type, unsigned char *keep, void *stream);

@@ -1,7 +1,7 @@
 /*
  * box_oracle.c -- CPU restatement of the reference's rotated-rectangle intersection
  * (Sutherland-Hodgman clip + shoelace area).  TEST INFRASTRUCTURE ONLY (see
- * pointnet2_oracle.c).  Follows /root/reference/utils/box_util.py:524-578
+ * pointnet2_oracle.c).  Follows reference utils/box_util.py:524-578
  * (helper_computeIntersection, helper_inside, polygon_clip_unnest) and the area
  * formula of :726-733, in fp32 like the TorchScript path the reference falls back
  * to when its Cython module is not compiled (utils/box_util.py:855-868).
@@ -28,13 +28,18 @@ static P2 intersect(P2 cp1, P2 cp2, P2 s, P2 e) {
   return r;
 }
 
+/* like the kernel (csrc/box_geometry.cuh), on the eight points taken relative to clip[0] */
 static float clipped_area(const P2 *subj, const P2 *clip) {
-  P2 a[16], b[16];
+  P2 a[16], b[16], cl[4];
   int na = 4;
-  memcpy(a, subj, sizeof(P2) * 4);
-  P2 cp1 = clip[3];
+  const P2 org = clip[0];
+  for (int i = 0; i < 4; ++i) {
+    a[i].x = subj[i].x - org.x; a[i].y = subj[i].y - org.y;
+    cl[i].x = clip[i].x - org.x; cl[i].y = clip[i].y - org.y;
+  }
+  P2 cp1 = cl[3];
   for (int ci = 0; ci < 4; ++ci) {
-    const P2 cp2 = clip[ci];
+    const P2 cp2 = cl[ci];
     int nb = 0;
     P2 s = a[na - 1];
     for (int i = 0; i < na; ++i) {

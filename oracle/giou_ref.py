@@ -50,10 +50,12 @@ def _intersect(cp1, cp2, s, e):
 
 
 def _clip_area(subj, clip):
-    out = [tuple(np.float32(v) for v in p) for p in subj]
-    cp1 = tuple(np.float32(v) for v in clip[-1])
-    for cv in clip:
-        cp2 = tuple(np.float32(v) for v in cv)
+    # like the kernel (csrc/box_geometry.cuh), on the eight points taken relative to clip[0]
+    org = tuple(np.float32(v) for v in clip[0])
+    out = [tuple(np.float32(v) - o for v, o in zip(p, org)) for p in subj]
+    clip = [tuple(np.float32(v) - o for v, o in zip(p, org)) for p in clip]
+    cp1 = clip[-1]
+    for cp2 in clip:
         inp, out = out, []
         s = inp[-1]
         for e in inp:
