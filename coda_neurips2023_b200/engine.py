@@ -15,6 +15,9 @@ object, laid out for the H100:
     (optimizer.py:4-36: `filter_biases_wd` -> no decay on 1-D parameters and biases) are per-range
     weight-decay values; parameters that never receive a gradient are left out of the update, as
     torch's AdamW skips `grad is None` parameters;
+  * the caller's torch.optim.AdamW can be adopted (`TrainStep(optimizer=...)`): its moments and step count are
+    imported into the flat buffers and its per-parameter state becomes views of them, so the reference's
+    save_checkpoint / resume_if_possible carry the optimizer state through unchanged;
   * rank 0's parameters and buffers are broadcast before the first step (what DDP's constructor does;
     the reference seeds every rank differently, main.py:982-985);
   * BatchNorm statistics stay per GPU (no SyncBatchNorm): the step's only other collective is the
@@ -26,6 +29,7 @@ from __future__ import annotations
 
 import ctypes
 import math
+import weakref
 
 import torch
 import torch.distributed as dist
@@ -218,14 +222,20 @@ class FlatAdamW:
         L = ops.lib()
         L.coda_grad_norm_scratch_floats.restype = ctypes.c_longlong
         self.scratch = torch.empty(int(L.coda_grad_norm_scratch_floats()), dtype=torch.float32, device=dev)
-        n = len(flat.params)
+        self.active = [True] * len(flat.params) if active is None else list(active)
+        raw, self.nchunks = self._chunk_table(weight_decay)
+        self.chunks = raw.to(dev)
+
+    def _chunk_table(self, weight_decay):
+        """(offset, len, weight_decay) of every CHUNK-element piece of the active parameters, as raw bytes."""
+        f = self.flat
+        n = len(f.params)
         wds = [float(weight_decay)] * n if not isinstance(weight_decay, (list, tuple)) else list(weight_decay)
-        active = [True] * n if active is None else list(active)
         chunks = []
-        for i, p in enumerate(flat.params):
-            if not active[i]:
+        for i, p in enumerate(f.params):
+            if not self.active[i]:
                 continue
-            off, left = flat.offsets[i], p.numel()
+            off, left = f.offsets[i], p.numel()
             while left > 0:
                 ln = min(left, self.CHUNK)
                 chunks.append((off, ln, wds[i]))
@@ -234,9 +244,12 @@ class FlatAdamW:
         arr = (self._Chunk * max(len(chunks), 1))()
         for k, (off, ln, wd) in enumerate(chunks):
             arr[k].offset, arr[k].len, arr[k].weight_decay = off, ln, wd
-        raw = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).clone()
-        self.chunks = raw.to(dev)
-        self.nchunks = len(chunks)
+        return torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).clone(), len(chunks)
+
+    def set_weight_decay(self, weight_decay):
+        """New per-parameter weight decay, written into the chunk table in place (a captured step reads it there)."""
+        raw, _ = self._chunk_table(weight_decay)
+        self.chunks.copy_(raw)
 
     def step(self, grad_scale: float = 1.0):
         f = self.flat
@@ -265,6 +278,151 @@ def _no_decay(name: str, p: torch.Tensor) -> bool:
     return p.dim() == 1 or name.endswith("bias")
 
 
+# ------------------------------------------------------------------ torch.optim.AdamW state <-> the flat layout
+# A torch optimizer's state_dict numbers its parameters in param_groups order; `index[i]` is that number for the i-th
+# parameter of a FlatParameters layout.  FlatAdamW keeps one step count for every parameter it updates (the active
+# ones); the moments of every parameter, inactive ones included, sit in its flat buffers at the parameter's offset.
+
+def _names(names, idx, most: int = 4) -> str:
+    picked = [names[i] for i in idx]
+    return ", ".join(picked[:most]) + (f" and {len(picked) - most} more" if len(picked) > most else "")
+
+
+def adamw_flat_index(optimizer, flat: FlatParameters) -> list:
+    """`index[i]`: the state_dict number of `flat.params[i]` in `optimizer`.  ValueError unless `optimizer` is a
+    torch.optim.AdamW over exactly the trainable parameters of the layout, each once."""
+    if not isinstance(optimizer, torch.optim.AdamW):
+        raise ValueError(f"TrainStep adopts a torch.optim.AdamW, not a {type(optimizer).__name__}")
+    ordered = [p for g in optimizer.param_groups for p in g["params"]]
+    number = {}
+    for k, p in enumerate(ordered):
+        number.setdefault(id(p), k)
+    mine = {id(p) for p in flat.params}
+    missing = [i for i, p in enumerate(flat.params) if id(p) not in number]
+    foreign = [k for k, p in enumerate(ordered) if id(p) not in mine]
+    if missing or foreign or len(number) != len(ordered):
+        raise ValueError("the optimizer's parameters must be exactly the model's trainable parameters: "
+                         + "; ".join(s for s in (
+                             f"not in the optimizer: {_names(flat.names, missing)}" if missing else "",
+                             f"{len(foreign)} optimizer parameters that are not trainable parameters of the model "
+                             f"(state_dict numbers {foreign[:8]})" if foreign else "",
+                             f"{len(ordered) - len(number)} listed twice" if len(number) != len(ordered) else "") if s))
+    return [number[id(p)] for p in flat.params]
+
+
+_ADAMW_RULE_OPTIONS = ("amsgrad", "maximize", "differentiable")
+
+
+def adamw_hyperparameters(param_groups, index: list):
+    """(weight decay of each parameter of the layout, betas, eps) from the optimizer's param_groups.  ValueError for
+    an option that changes the update rule, and for betas / eps that differ between groups (the flat step has one
+    of each)."""
+    for g_i, g in enumerate(param_groups):
+        bad = [k for k in _ADAMW_RULE_OPTIONS if g.get(k, False)]
+        if not g.get("decoupled_weight_decay", True):
+            bad.append("decoupled_weight_decay=False")
+        if bad:
+            raise ValueError(f"param_groups[{g_i}] sets {', '.join(bad)}: the flat step implements plain AdamW")
+    rules = {(tuple(float(b) for b in g["betas"]), float(g["eps"])) for g in param_groups}
+    if len(rules) != 1:
+        raise ValueError(f"param_groups differ in betas / eps {sorted(rules)}: the flat step takes one of each")
+    (betas, eps), = rules
+    decay = [float(g["weight_decay"]) for g in param_groups for _ in g["params"]]
+    return [decay[k] for k in index], betas, eps
+
+
+def adamw_state_to_flat(state: dict, index: list, flat: FlatParameters, active: list, exp_avg: torch.Tensor,
+                        exp_avg_sq: torch.Tensor):
+    """Copies the per-parameter moments of `state` (a state_dict's "state": number -> {"step", "exp_avg",
+    "exp_avg_sq"}) into the flat moment buffers, zero elsewhere.  Returns (the active parameters' common step count,
+    0 without state; {i: step} of the inactive parameters that have state, carried unchanged).  Everything is checked
+    before anything is written: ValueError for a state entry without a step count, for moments that do not fit their
+    parameter, for active parameters with different step counts, or for state on some active parameters but not on
+    others.  The moments may be views of the flat buffers themselves (an optimizer that reloads its own state_dict
+    in memory keeps them: torch's load_state_dict does not copy a tensor that is already on the right device)."""
+    steps = {}
+    for i, p in enumerate(flat.params):
+        st = state.get(index[i])
+        if not st:
+            continue
+        if "step" not in st:
+            raise ValueError(f"optimizer state of {flat.names[i]} has no step count")
+        for key in ("exp_avg", "exp_avg_sq"):
+            if key not in st or tuple(st[key].shape) != tuple(p.shape):
+                got = tuple(st[key].shape) if key in st else "none"
+                raise ValueError(f"optimizer state of {flat.names[i]}: {key} {got} does not fit the parameter "
+                                 f"{tuple(p.shape)}")
+        steps[i] = float(st["step"])
+    act = [i for i, a in enumerate(active) if a]
+    with_state = [i for i in act if i in steps]
+    if with_state and len(with_state) != len(act):
+        without = [i for i in act if i not in steps]
+        raise ValueError("the optimizer holds state for some of the parameters that receive a gradient but not for "
+                         f"others (with: {_names(flat.names, with_state)}; without: {_names(flat.names, without)}); "
+                         "the flat step keeps one step count for all of them")
+    counts = sorted({steps[i] for i in with_state})
+    if len(counts) > 1:
+        first = {s: next(i for i in with_state if steps[i] == s) for s in counts}
+        raise ValueError("the parameters that receive a gradient have different AdamW step counts ("
+                         + ", ".join(f"{flat.names[i]}: {s:g}" for s, i in first.items())
+                         + "); the flat step keeps one step count for all of them")
+    own = {exp_avg.untyped_storage().data_ptr(), exp_avg_sq.untyped_storage().data_ptr()}
+
+    def source(t):      # read before the buffers are cleared
+        return t.clone() if t.untyped_storage().data_ptr() in own else t
+
+    with torch.no_grad():
+        sources = {i: (source(state[index[i]]["exp_avg"]), source(state[index[i]]["exp_avg_sq"])) for i in steps}
+        exp_avg.zero_()
+        exp_avg_sq.zero_()
+        for i, (m, v) in sources.items():
+            off, n = flat.offsets[i], flat.params[i].numel()
+            exp_avg[off:off + n].copy_(m.reshape(-1))
+            exp_avg_sq[off:off + n].copy_(v.reshape(-1))
+    return (counts[0] if counts else 0.0), {i: s for i, s in steps.items() if not active[i]}
+
+
+def adamw_state_from_flat(param_groups, index: list, flat: FlatParameters, active: list, exp_avg: torch.Tensor,
+                          exp_avg_sq: torch.Tensor, step: float, carried: dict) -> dict:
+    """The inverse: a state_dict's "state" whose moments are VIEWS of the flat buffers.  Active parameters have state
+    once `step` > 0 (torch creates it on the first update); inactive ones where `carried` has their step.  `step` is
+    a float32 tensor on the CPU, or on the parameter's device for capturable / fused groups, as torch keeps it."""
+    on_device = [bool(g.get("capturable", False) or g.get("fused", False)) for g in param_groups for _ in g["params"]]
+    state = {}
+    for i, p in enumerate(flat.params):
+        s = step if active[i] else carried.get(i)
+        if s is None or (active[i] and s <= 0):
+            continue
+        off, n = flat.offsets[i], p.numel()
+        state[index[i]] = {
+            "step": torch.tensor(float(s), dtype=torch.float32, device=p.device if on_device[index[i]] else "cpu"),
+            "exp_avg": exp_avg[off:off + n].view_as(p),
+            "exp_avg_sq": exp_avg_sq[off:off + n].view_as(p)}
+    return dict(sorted(state.items()))
+
+
+def bind_adamw_state(optimizer, index: list, flat: FlatParameters, active: list, exp_avg: torch.Tensor,
+                     exp_avg_sq: torch.Tensor, step: float, carried: dict) -> None:
+    """Replaces the optimizer's per-parameter state by `adamw_state_from_flat`: its state_dict() then reads the flat
+    buffers."""
+    state = adamw_state_from_flat(optimizer.param_groups, index, flat, active, exp_avg, exp_avg_sq, step, carried)
+    for k, p in enumerate(p for g in optimizer.param_groups for p in g["params"]):
+        if k in state:
+            optimizer.state[p] = state[k]
+        else:
+            optimizer.state.pop(p, None)
+
+
+# adopted optimizer -> (the TrainStep that holds it, the handles of its state_dict / load_state_dict hooks)
+_ADOPTED = weakref.WeakKeyDictionary()
+
+
+def adamw_numbered_state(optimizer) -> dict:
+    """optimizer.state keyed by state_dict number (what state_dict() packs, without running its hooks)."""
+    ordered = [p for g in optimizer.param_groups for p in g["params"]]
+    return {k: optimizer.state[p] for k, p in enumerate(ordered) if optimizer.state.get(p)}
+
+
 class TrainStep:
     """The step runs either eagerly or, after `capture()`, as ONE CUDA graph: the ~6 000 kernel
     launches of a step (8 decoder layers x many small ops) are launch-bound on the host otherwise.
@@ -278,12 +436,22 @@ class TrainStep:
     state is broadcast, the optimizer is built.  The probe and the graph warm-up leave NO trace: parameters,
     optimizer state, BatchNorm buffers and the dropout counter are restored afterwards."""
 
-    def __init__(self, args, model, criterion, device, nbuckets: int = 4, sync_bn: bool | None = None):
+    def __init__(self, args, model, criterion, device, nbuckets: int = 4, sync_bn: bool | None = None,
+                 optimizer: torch.optim.AdamW | None = None):
         """sync_bn: synchronise BatchNorm statistics over the ranks (the reference converts to SyncBatchNorm when
         ngpus > 1, main.py:993).  Default (None -> args.sync_bn, else False): per-GPU statistics and exactly one
         gradient all-reduce per step, as the north-star asks; True adds one small all-reduce per BatchNorm layer
-        and direction (DESIGN.md section 7) and makes N ranks x B scenes equal one rank x N*B scenes."""
+        and direction (DESIGN.md section 7) and makes N ranks x B scenes equal one rank x N*B scenes.
+
+        optimizer: the caller's torch.optim.AdamW over the model's trainable parameters (the reference's
+        build_optimizer), possibly holding a loaded state.  `prepare` adopts it: its moments and step count become
+        the flat step's, its per-group weight decay, betas and eps replace the values derived from `args` (the
+        learning rate still follows the schedule), and its per-parameter moments become views of the flat buffers,
+        so that its state_dict() is what the step runs with and a later load_state_dict() is what it runs on.  The
+        optimizer's hooks keep this step alive as long as the optimizer lives; a step that adopts the same optimizer
+        later takes it over."""
         self.args, self.model, self.criterion, self.device = args, model, criterion, device
+        self.adamw = optimizer
         self.world = get_world_size()
         self.sync_bn = bool(getattr(args, "sync_bn", False) if sync_bn is None else sync_bn)
         ops.set_bn_sync(self.sync_bn and self.world > 1)
@@ -413,6 +581,18 @@ class TrainStep:
         for name, p in zip(self.flat.names, self.flat.params):
             wds.append(0.0 if (getattr(a, "filter_biases_wd", False) and _no_decay(name, p)) else float(a.weight_decay))
         self.optimizer = FlatAdamW(self.flat, self.lr, wds, active, max_norm=float(a.clip_gradient))
+        if self.adamw is not None:
+            # one step at a time holds an optimizer: a step that adopts it later takes it over, from the step count
+            # the holder has reached (the optimizer's own copy is refreshed only when a state_dict is taken)
+            holder = _ADOPTED.get(self.adamw)
+            if holder is not None:
+                holder[0]._export()
+            self._adopt_on_every_rank()
+            if holder is not None:
+                for h in holder[1]:
+                    h.remove()
+            _ADOPTED[self.adamw] = (self, (self.adamw.register_state_dict_pre_hook(lambda _opt: self._export()),
+                                           self.adamw.register_load_state_dict_post_hook(self._reload)))
         self.reducer = BucketedAllReduce(self.flat, self.nbuckets, active)
         self.inactive_names = [n for n, f in zip(self.flat.names, active) if not f]
         # from now on the backward kernels write single-use parameter gradients straight into flat_grad
@@ -430,6 +610,78 @@ class TrainStep:
             self.flat.zero_grad()
             ops.invalidate_weight_cache()
         return self
+
+    # ------------------------------------------------------------------ the caller's AdamW
+    def _adopt(self):
+        """The adopted optimizer's options, moments and step count -> FlatAdamW; then its state is bound to the flat
+        buffers.  Every check runs before FlatAdamW changes."""
+        fa, opt = self.optimizer, self.adamw
+        index = adamw_flat_index(opt, self.flat)
+        wds, betas, eps = adamw_hyperparameters(opt.param_groups, index)
+        if self.graph is not None and (betas, eps) != (tuple(fa.betas), fa.eps):
+            raise ValueError(f"betas {betas} / eps {eps} differ from the captured step's {tuple(fa.betas)} / {fa.eps}: "
+                             "load the optimizer state before capture")
+        step, carried = adamw_state_to_flat(adamw_numbered_state(opt), index, self.flat, fa.active, fa.exp_avg,
+                                            fa.exp_avg_sq)
+        fa.state[0].fill_(step)
+        fa.set_weight_decay(wds)
+        fa.betas, fa.eps = betas, eps
+        self._adamw_index, self._carried = index, carried
+        self._adamw_groups = [{k: v for k, v in g.items() if k not in ("params", "lr")} for g in opt.param_groups]
+        self._export(step)
+
+    def _export(self, step: float | None = None):
+        """Binds the adopted optimizer's per-parameter state to the flat buffers.  Without `step`, the step count is
+        read from the device: the one device -> host read of a state_dict(), none per step."""
+        fa = self.optimizer
+        if step is None:
+            step = float(fa.state[0])
+        bind_adamw_state(self.adamw, self._adamw_index, self.flat, fa.active, fa.exp_avg, fa.exp_avg_sq, step,
+                         self._carried)
+
+    def _reload(self, opt):
+        """After optimizer.load_state_dict: import the loaded state in place (a captured step reads the flat buffers,
+        no re-capture).  If it is refused, the optimizer goes back to describing the state the step runs with."""
+        try:
+            self._adopt()
+        except ValueError:
+            for g, kept in zip(opt.param_groups, self._adamw_groups):
+                g.update(kept)
+            self._export()
+            raise
+
+    def _adopt_on_every_rank(self):
+        """`_adopt` at prepare.  With several ranks, all of them learn whether any rank refused its optimizer state
+        before rank 0's state is broadcast: a refusal on one rank alone would leave the others waiting in the
+        broadcast."""
+        err = None
+        try:
+            self._adopt()
+        except ValueError as e:
+            err = e
+        if is_distributed() and self.world > 1:
+            refused = torch.zeros(self.world, device=self.device)
+            refused[dist.get_rank()] = float(err is not None)
+            dist.all_reduce(refused)
+            ranks = refused.nonzero().flatten().tolist()
+            if ranks:
+                raise err or ValueError(f"the optimizer state was refused on rank(s) {ranks}")
+            self._broadcast_adopted()
+        elif err is not None:
+            raise err
+
+    def _broadcast_adopted(self):
+        """Rank 0's moments and step counts on every rank (DDP-constructor semantics, as for the parameters)."""
+        fa = self.optimizer
+        for t in (fa.exp_avg, fa.exp_avg_sq, fa.state):
+            dist.broadcast(t, 0)
+        inactive = [i for i, f in enumerate(fa.active) if not f]
+        if inactive:
+            steps = torch.tensor([self._carried.get(i, -1.0) for i in inactive], dtype=torch.float64,
+                                 device=self.device)
+            dist.broadcast(steps, 0)
+            self._carried = {i: s for i, s in zip(inactive, steps.tolist()) if s >= 0}
+        self._export()
 
     def capture(self, example_batch: dict, warmup: int = 3, curr_epoch: float = 0.0):
         """Captures the whole step into a CUDA graph (static copy of `example_batch` as input).  The warm-up
