@@ -1,5 +1,5 @@
 // Evaluation path on the device (sm_90a): what the reference's APCalculator does box by box on the host with numpy /
-// scipy (utils/ap_calculator.py, utils/nms.py, utils/eval_det.py, utils/box_util.py) as four batched kernels.
+// scipy (utils/ap_calculator.py, utils/nms.py, utils/eval_det.py, utils/box_util.py) as batched kernels.
 //
 //   points_in_boxes   -- "remove_empty_box": how many points of the scene lie inside each predicted box
 //                        (ap_calculator.py:808-835: a scipy Delaunay hull test per box; here three dot products
@@ -10,6 +10,10 @@
 //                        (utils/box_util.py:156-183, called pair by pair from utils/eval_det.py:122-130)
 //   eval_match        -- VOC matching per (scene, class): detections in descending score order claim the ground-truth
 //                        box of their class they overlap most (utils/eval_det.py:110-146)
+//   eval_records      -- the accumulated (score, true-positive) results of a step as compact detection records, which
+//                        ranks can exchange and merge
+//   eval_ap           -- cumulative TP / FP, precision, recall, envelope and VOC AP of every (class, IoU threshold)
+//                        over the sorted records (utils/eval_det.py:147-162, voc_ap :23-55), one launch
 // Nothing here synchronises with the host; a whole evaluation step is five launches.  C-ABI in include/coda_eval.h.
 #include <math.h>
 #include <stdint.h>
@@ -258,6 +262,181 @@ eval_match_kernel(int k, int g, int ncls, const float *__restrict__ iou, const f
   }
 }
 
+// ------------------------------------------------------------------ detection records
+// One thread per (scene, box, class) of a step, class fastest (the layout of scores).  A live, finitely scored entry
+// becomes a record; the warp takes its slots with one atomic on the shared counter.  Slots are handed out in no
+// particular order -- the sort that follows fixes it.
+__global__ void __launch_bounds__(256)
+eval_records_kernel(long long n, int b, int k, int ncls, int nthr, long long scene_base,
+                    const float *__restrict__ scores, const unsigned char *__restrict__ det_mask,
+                    const unsigned char *__restrict__ tp, int *__restrict__ counter, int capacity,
+                    int *__restrict__ rec_cls, float *__restrict__ rec_score, long long *__restrict__ rec_pos,
+                    unsigned *__restrict__ rec_tp) {
+  const int lane = threadIdx.x & 31;
+  // the loop bound is uniform over the block, so every lane reaches every ballot
+  for (long long base = (long long)blockIdx.x * blockDim.x; base < n; base += (long long)gridDim.x * blockDim.x) {
+    const long long idx = base + threadIdx.x;
+    int c = 0, j = 0, bb = 0;
+    float s = 0.f;
+    bool ok = false;
+    if (idx < n) {
+      c = (int)(idx % ncls);
+      const long long bj = idx / ncls;
+      j = (int)(bj % k);
+      bb = (int)(bj / k);
+      s = scores[idx];
+      ok = det_mask[bj] != 0 && isfinite(s);
+    }
+    const unsigned ballot = __ballot_sync(0xffffffffu, ok);
+    if (ballot == 0u) continue;
+    int first = 0;
+    if (lane == __ffs(ballot) - 1) first = atomicAdd(counter, __popc(ballot));
+    first = __shfl_sync(0xffffffffu, first, __ffs(ballot) - 1);
+    if (!ok) continue;
+    const long long slot = (long long)first + __popc(ballot & ((1u << lane) - 1u));
+    if (slot >= capacity) continue;          // the caller sees the counter pass the capacity
+    unsigned m = 0u;
+    for (int t = 0; t < nthr; ++t)
+      m |= (tp[(((size_t)t * b + bb) * ncls + c) * k + j] != 0 ? 1u : 0u) << t;
+    rec_cls[slot] = c;
+    rec_score[slot] = s == 0.f ? 0.f : s;    // -0 and +0 are one score: the sort key must not tell them apart
+    rec_pos[slot] = (scene_base + bb) * k + j;
+    rec_tp[slot] = m;
+  }
+}
+
+// ------------------------------------------------------------------ per-class precision / recall / VOC AP
+// One CTA per (class, IoU threshold) over the class's segment of the sorted records (utils/eval_det.py:147-162 and
+// voc_ap, :23-55, use_07_metric=False).  With cum_i the true positives among records 0..i of the segment and npos
+// the class's ground-truth boxes:
+//   prec_i = cum_i / (i + 1),  rec_i = cum_i / npos (0 if npos == 0),  env_i = max_{j >= i} prec_j,
+//   AP = sum over the records where the recall steps (tp_i = 1, npos > 0) of (rec_i - rec_{i-1}) * env_i.
+// voc_ap's end points add nothing: mrec = 1 after the last record pairs with mpre = 0.  The envelope is a suffix
+// maximum, so the segment is walked from its end in chunks of AP_THREADS x AP_ITEMS records, each a block scan that
+// carries (true positives after the chunk, envelope after the chunk) into the next; a first pass counts the segment's
+// true positives, from which cum_i follows.  Counts are exact in fp64, and prec / rec are the same correctly rounded
+// divisions numpy performs; only the AP sum is taken in another order.
+constexpr int AP_THREADS = 256;
+constexpr int AP_ITEMS = 8;
+constexpr int AP_CHUNK = AP_THREADS * AP_ITEMS;
+constexpr int AP_WARPS = AP_THREADS / 32;
+
+struct AddOp {
+  template <typename T> __device__ __forceinline__ T operator()(T a, T b) const { return a + b; }
+};
+struct MaxOp {
+  __device__ __forceinline__ double operator()(double a, double b) const { return fmax(a, b); }
+};
+
+// exclusive scan over the block in thread order; `identity` for thread 0, the block's total in `total`
+template <typename T, typename Op>
+__device__ __forceinline__ T block_exclusive_scan(T v, T identity, Op op, T *sh, T &total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  T inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const T u = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc = op(inc, u);
+  }
+  if (lane == 31) sh[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    T w = lane < AP_WARPS ? sh[lane] : identity;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const T u = __shfl_up_sync(0xffffffffu, w, o);
+      if (lane >= o) w = op(w, u);
+    }
+    if (lane < AP_WARPS) sh[lane] = w;
+  }
+  __syncthreads();
+  T ex = __shfl_up_sync(0xffffffffu, inc, 1);
+  if (lane == 0) ex = identity;
+  if (warp > 0) ex = op(sh[warp - 1], ex);
+  total = sh[AP_WARPS - 1];
+  __syncthreads();                           // sh is reused by the next scan
+  return ex;
+}
+
+__global__ void __launch_bounds__(AP_THREADS)
+eval_ap_kernel(int ncls, long long nrec, const long long *__restrict__ offsets, const unsigned *__restrict__ rec_tp,
+               const long long *__restrict__ npos, double *__restrict__ ap, double *__restrict__ last_prec,
+               double *__restrict__ last_rec, double *__restrict__ curves) {
+  __shared__ int sh_i[AP_WARPS];
+  __shared__ double sh_d[AP_WARPS];
+  const int c = blockIdx.x, t = blockIdx.y;
+  const long long lo = offsets[c], n = offsets[c + 1] - lo;
+  const long long np = npos[c];
+  const double dnp = (double)np;
+  const unsigned *seg = rec_tp + lo;
+
+  int mine = 0;
+  for (long long i = threadIdx.x; i < n; i += AP_THREADS) mine += (seg[i] >> t) & 1u;
+  int total;
+  block_exclusive_scan(mine, 0, AddOp(), sh_i, total);
+
+  int after_tp = 0;                          // true positives of the records behind the current chunk
+  double after_env = 0.0;                    // largest precision among them (voc_ap pads the envelope with 0)
+  double acc = 0.0;
+  for (long long hi = n; hi > 0; hi -= AP_CHUNK) {
+    // this thread's records, walked backwards: q = 0 is the one nearest the segment's end
+    const long long top = hi - 1 - (long long)threadIdx.x * AP_ITEMS;
+    const long long chunk_lo = hi > AP_CHUNK ? hi - AP_CHUNK : 0;
+    unsigned bits = 0u;
+    int run = 0;
+#pragma unroll
+    for (int q = 0; q < AP_ITEMS; ++q) {
+      const long long i = top - q;
+      const unsigned b = (i >= chunk_lo) ? (seg[i] >> t) & 1u : 0u;
+      bits |= b << q;
+      run += (int)b;
+    }
+    int chunk_tp;
+    const int later = block_exclusive_scan(run, 0, AddOp(), sh_i, chunk_tp);   // chunk records after this thread's
+    double prec[AP_ITEMS], rise[AP_ITEMS];  // rise: rec_i - rec_{i-1}, 0 where the recall does not step
+    double pmax = 0.0;
+    int suffix = after_tp + later;          // true positives at or after record i
+#pragma unroll
+    for (int q = 0; q < AP_ITEMS; ++q) {
+      const long long i = top - q;
+      const int b = (bits >> q) & 1u;
+      suffix += b;
+      const long long cum = (long long)total - suffix + b;
+      prec[q] = 0.0;
+      rise[q] = 0.0;
+      if (i >= chunk_lo) {
+        prec[q] = (double)cum / (double)(i + 1);
+        pmax = fmax(pmax, prec[q]);
+        if (b && np > 0) rise[q] = (double)cum / dnp - (double)(cum - 1) / dnp;
+        if (curves) {
+          const size_t row = (size_t)t * 4 * nrec + (size_t)(lo + i);
+          curves[row] = (double)cum;
+          curves[row + nrec] = (double)(i + 1 - cum);
+          curves[row + 2 * (size_t)nrec] = np > 0 ? (double)cum / dnp : 0.0;
+          curves[row + 3 * (size_t)nrec] = prec[q];
+        }
+      }
+    }
+    double chunk_max;
+    double env = fmax(after_env, block_exclusive_scan(pmax, 0.0, MaxOp(), sh_d, chunk_max));
+#pragma unroll
+    for (int q = 0; q < AP_ITEMS; ++q) {
+      env = fmax(env, prec[q]);
+      if (rise[q] != 0.0) acc += rise[q] * env;
+    }
+    after_tp += chunk_tp;
+    after_env = fmax(after_env, chunk_max);
+  }
+  double sum;
+  block_exclusive_scan(acc, 0.0, AddOp(), sh_d, sum);
+  if (threadIdx.x == 0) {
+    const int o = t * ncls + c;
+    ap[o] = sum;
+    last_prec[o] = n > 0 ? (double)total / (double)n : 0.0;
+    last_rec[o] = (n > 0 && np > 0) ? (double)total / dnp : 0.0;
+  }
+}
+
 }  // namespace
 
 extern "C" {
@@ -315,6 +494,31 @@ int coda_eval_match(int b, int k, int g, int ncls, const float *iou, const float
   }
   eval_match_kernel<<<dim3((ncls + wpb - 1) / wpb, b), wpb * 32, smem, (cudaStream_t)stream>>>(
       k, g, ncls, iou, scores, det_mask, gt_cls, gt_present, iou_thresh, tp);
+  return launch_status();
+}
+
+int coda_eval_records(int b, int k, int ncls, int nthr, long long scene_base, const float *scores,
+                      const unsigned char *det_mask, const unsigned char *tp, int *counter, int capacity,
+                      int *rec_cls, float *rec_score, long long *rec_pos, unsigned *rec_tp, void *stream) {
+  if (b < 0 || k < 0 || ncls < 0 || nthr < 1 || nthr > 32 || scene_base < 0 || capacity < 0) return CODA_EINVAL;
+  if (b == 0 || k == 0 || ncls == 0) return CODA_OK;
+  if (!scores || !det_mask || !tp || !counter || (capacity > 0 && (!rec_cls || !rec_score || !rec_pos || !rec_tp)))
+    return CODA_EINVAL;
+  const long long n = (long long)b * k * ncls;
+  const long long blocks = (n + 255) / 256;
+  eval_records_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, (cudaStream_t)stream>>>(
+      n, b, k, ncls, nthr, scene_base, scores, det_mask, tp, counter, capacity, rec_cls, rec_score, rec_pos, rec_tp);
+  return launch_status();
+}
+
+int coda_eval_ap(int ncls, int nthr, long long nrec, const long long *offsets, const unsigned *rec_tp,
+                 const long long *npos, double *ap, double *last_prec, double *last_rec, double *curves,
+                 void *stream) {
+  if (ncls < 0 || nthr < 1 || nthr > 32 || nrec < 0) return CODA_EINVAL;
+  if (ncls == 0) return CODA_OK;
+  if (!offsets || !npos || !ap || !last_prec || !last_rec || (nrec > 0 && !rec_tp)) return CODA_EINVAL;
+  eval_ap_kernel<<<dim3(ncls, nthr), AP_THREADS, 0, (cudaStream_t)stream>>>(ncls, nrec, offsets, rec_tp, npos, ap,
+                                                                          last_prec, last_rec, curves);
   return launch_status();
 }
 

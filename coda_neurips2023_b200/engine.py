@@ -777,22 +777,32 @@ def evaluate(args, curr_epoch, model, criterion, dataset_config, dataset_loader,
     """Evaluation loop (reference engine.py:2553-2661): model in eval mode -> (optional loss) -> APCalculator.
     Differences are implementation-only: the AP bookkeeping of a batch runs on the device (utils/ap_calculator.py,
     five kernel launches, no host copies), and under data parallelism the ranks do not all-gather their point
-    clouds and outputs (`all_gather_dict`, :2634-2636) -- each rank matches its own scenes and only the (score,
-    true-positive) records would have to be gathered; call `compute_metrics()` on the returned calculator."""
+    clouds and outputs (`all_gather_dict`, :2634-2636): the calculator is rank-local, each rank matches its own
+    scenes, and `compute_metrics()` on the returned calculator is a collective that exchanges the detection records --
+    every rank must call it.  The loss is averaged over the ranks as the reference does."""
     from .utils.ap_calculator import APCalculator
+    from .utils.dist import all_reduce_average, get_rank, reduce_dict
 
+    world = get_world_size()
     ap_calculator = APCalculator(dataset_config=dataset_config, ap_iou_thresh=[0.25, 0.5],
-                                 class2type_map=getattr(dataset_config, "class2type", None), exact_eval=True, args=args)
+                                 class2type_map=getattr(dataset_config, "class2type", None), exact_eval=True, args=args,
+                                 rank=get_rank(), world_size=world)
     device = next(model.parameters()).device
     model.eval()
     loss_sum, nloss = 0.0, 0
+    loss_dict_reduced = None
     for batch in dataset_loader:
         batch = {k: (v.to(device, non_blocking=True) if isinstance(v, torch.Tensor) else v) for k, v in batch.items()}
         outputs = model(batch, if_real_test=if_real_test, if_cmp_class=if_cmp_class)
         if criterion is not None:
-            loss, _ = criterion(outputs, batch)
+            loss, loss_dict = criterion(outputs, batch)
+            if world > 1:
+                loss = all_reduce_average(loss)
+                loss_dict_reduced = reduce_dict(loss_dict)
             loss_sum, nloss = loss_sum + loss.detach(), nloss + 1
         ap_calculator.step_meter(outputs, batch)
     if logger is not None and nloss and is_primary():
+        if loss_dict_reduced is not None:
+            logger.log_scalars(loss_dict_reduced, curr_train_iter, prefix="Test_details/")
         logger.log_scalars({"loss": float(loss_sum) / nloss}, curr_train_iter, prefix="Test/")
     return ap_calculator

@@ -11,13 +11,17 @@ five kernel launches (include/coda_eval.h) on the batch as it leaves the model -
     points_in_boxes -> non-empty mask | nms3d (same-class / class-agnostic) | box3d_iou (B, K, G) |
     eval_match per IoU threshold -> tp (B, C, K)
 
-Per class, precision / recall / VOC AP are then computed from all accumulated (score, tp) exactly as
-utils/eval_det.py:147-162 + voc_ap (:23-55).
+`compute_metrics` compacts what the steps accumulated into one record per (scene, box, class) detection
+(`coda_eval_records`), sorts the records by (class, score descending, scene and box), and computes precision / recall /
+VOC AP of every class and IoU threshold in one launch (`coda_eval_ap`) as utils/eval_det.py:147-162 + voc_ap (:23-55)
+do.  Records are what data-parallel ranks exchange: a rank-local calculator scores only its own scenes and merges the
+other ranks' records in `compute_metrics`, instead of gathering every point cloud and output before each step.
 """
 from __future__ import annotations
 
 import ctypes
 from collections import OrderedDict
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -101,6 +105,132 @@ def eval_match(iou: torch.Tensor, scores: torch.Tensor, det_mask: torch.Tensor, 
                                    _f(iou_thresh), ptr(tp), stream_of(scores))
     check(st, "eval_match")
     return tp.bool()
+
+
+class EvalRecords(NamedTuple):
+    """One record per (scene, box, class) detection: class int32, score fp32, global position int64 (scene x K + box,
+    the order that breaks score ties), tp int32 (bit t = true positive at IoU threshold t)."""
+    cls: torch.Tensor
+    score: torch.Tensor
+    pos: torch.Tensor
+    tp: torch.Tensor
+
+    def __len__(self):
+        return self.cls.shape[0]
+
+
+def eval_records(scores: list, det_masks: list, tps: list, scene_bases: list) -> EvalRecords:
+    """Compacts accumulated steps -- scores (B, K, C) f32 (-inf / NaN = no detection), det_mask (B, K) bool,
+    tp (T, B, C, K) bool and the global number of each step's first scene -- into detection records, in no
+    particular order."""
+    dev = scores[0].device
+    cap = sum(s.numel() for s in scores)
+    rec = EvalRecords(torch.empty(cap, dtype=torch.int32, device=dev), torch.empty(cap, dtype=torch.float32, device=dev),
+                      torch.empty(cap, dtype=torch.int64, device=dev), torch.empty(cap, dtype=torch.int32, device=dev))
+    counter = torch.zeros(1, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        for s, m, t, base in zip(scores, det_masks, tps, scene_bases):
+            b, k, c = s.shape
+            s, m, t = s.float().contiguous(), _bytes(m), _bytes(t)
+            st = lib().coda_eval_records(_i(b), _i(k), _i(c), _i(t.shape[0]), ctypes.c_longlong(int(base)), ptr(s),
+                                         ptr(m), ptr(t), ptr(counter), _i(cap), ptr(rec.cls), ptr(rec.score),
+                                         ptr(rec.pos), ptr(rec.tp), stream_of(s))
+            check(st, "eval_records")
+    n = int(counter.item())
+    if n > cap:
+        raise RuntimeError(f"eval_records: {n} records for a capacity of {cap}")
+    return EvalRecords(*(f[:n] for f in rec))
+
+
+def _bytes(t: torch.Tensor) -> torch.Tensor:
+    t = t.contiguous()
+    return t.view(torch.uint8) if t.dtype == torch.bool else t.to(torch.uint8)
+
+
+def pack_records(rec: EvalRecords) -> torch.Tensor:
+    """Records as one (n, 5) int32 block for an exchange between ranks: class, score bits, position (low word, high
+    word), tp mask."""
+    pos = rec.pos.long()
+    return torch.stack([rec.cls.int(), rec.score.float().view(torch.int32), (pos & 0xFFFFFFFF).int(),
+                        (pos >> 32).int(), rec.tp.int()], dim=1)
+
+
+def unpack_records(block: torch.Tensor) -> EvalRecords:
+    """Inverse of `pack_records`, for a block of any strides (a row slice of a padded exchange buffer)."""
+    block = block.to(torch.int32)
+    pos = (block[:, 3].long() << 32) | (block[:, 2].long() & 0xFFFFFFFF)
+    return EvalRecords(block[:, 0].contiguous(), block[:, 1].contiguous().view(torch.float32), pos.contiguous(),
+                       block[:, 4].contiguous())
+
+
+def merge_records(parts: list) -> EvalRecords:
+    """The records of several ranks as one set (the order is fixed later by `sort_records`)."""
+    return EvalRecords(*(torch.cat(f) for f in zip(*parts)))
+
+
+def sort_records(rec: EvalRecords) -> EvalRecords:
+    """Sorted by (class ascending, score descending, global position ascending): what a stable descending argsort
+    of each class's scores over the step-ordered (scene, box) rows gives."""
+    order = torch.sort(rec.pos, stable=True).indices
+    rec = EvalRecords(*(f[order] for f in rec))
+    # fp32 bits -> an unsigned key that ascends with the score, then flipped so that it descends
+    score = torch.where(rec.score == 0, torch.zeros_like(rec.score), rec.score)      # -0 ties with +0
+    u = score.view(torch.int32).long() & 0xFFFFFFFF
+    asc = torch.where(u >= 0x80000000, u ^ 0xFFFFFFFF, u | 0x80000000)
+    key = (rec.cls.long() << 32) | (0xFFFFFFFF - asc)
+    order = torch.sort(key, stable=True).indices
+    return EvalRecords(*(f[order] for f in rec))
+
+
+def eval_ap(rec: EvalRecords, ncls: int, nthr: int, npos: torch.Tensor, curves: bool = False):
+    """Per (threshold, class) VOC AP, last precision and last recall, (T, C) fp64 each, from records sorted by
+    `sort_records` and the per-class ground-truth counts npos (C,); with curves=True also the (T, 4, N) cumulative TP,
+    cumulative FP, recall and precision of every record.  Returns (ap, last_prec, last_rec, per-class record counts
+    (C,) int64, curves or None)."""
+    dev = npos.device
+    counts = torch.bincount(rec.cls.long(), minlength=ncls) if len(rec) else torch.zeros(ncls, dtype=torch.int64,
+                                                                                       device=dev)
+    offsets = torch.zeros(ncls + 1, dtype=torch.int64, device=dev)
+    torch.cumsum(counts, 0, out=offsets[1:])
+    npos = npos.to(torch.int64).contiguous()
+    tp = rec.tp.contiguous()
+    ap, last_prec, last_rec = (torch.empty((nthr, ncls), dtype=torch.float64, device=dev) for _ in range(3))
+    cur = torch.empty((nthr, 4, len(rec)), dtype=torch.float64, device=dev) if curves else None
+    with torch.cuda.device(dev):
+        st = lib().coda_eval_ap(_i(ncls), _i(nthr), ctypes.c_longlong(len(rec)), ptr(offsets), ptr(tp), ptr(npos),
+                                ptr(ap), ptr(last_prec), ptr(last_rec), ptr(cur), stream_of(npos))
+    check(st, "eval_ap")
+    return ap, last_prec, last_rec, counts, cur
+
+
+class RankState(NamedTuple):
+    """What a calculator has accumulated, in the form ranks exchange: detection records, ground-truth boxes per class
+    (C,) int64, first occurrence of each class among the predictions / the ground truth (C,) int64 (int64 max = never),
+    and the batch size of every step."""
+    records: EvalRecords
+    gt_count: torch.Tensor
+    first_pred: torch.Tensor
+    first_gt: torch.Tensor
+    batch_sizes: list
+
+
+def _check_batch_sizes(per_rank: list) -> None:
+    if any(list(s) != list(per_rank[0]) for s in per_rank[1:]):
+        raise ValueError("data-parallel evaluation needs every rank to hold the same number of scenes at every step; "
+                         f"per-rank batch sizes: {[list(s) for s in per_rank]}")
+
+
+def merge_rank_states(states: list) -> RankState:
+    """The states of W rank-local calculators (rank order) as the state of one calculator that saw every rank's
+    scenes: records merged, ground-truth counts summed, first occurrences reduced by minimum.  Raises ValueError when
+    the ranks' batch sizes differ at some step (the scene numbering assumes they do not)."""
+    _check_batch_sizes([s.batch_sizes for s in states])
+    live = [s for s in states if s.gt_count is not None]
+    if not live:
+        return states[0]
+    return RankState(merge_records([s.records for s in live]), torch.stack([s.gt_count for s in live]).sum(0),
+                     torch.stack([s.first_pred for s in live]).amin(0), torch.stack([s.first_gt for s in live]).amin(0),
+                     list(states[0].batch_sizes))
 
 
 # --------------------------------------------------------------------------- prediction parsing
@@ -198,10 +328,17 @@ def voc_ap(rec, prec, use_07_metric=False):
 
 
 class APCalculator(object):
-    """Calculating Average Precision (reference utils/ap_calculator.py:1054-1810), on the device."""
+    """Calculating Average Precision (reference utils/ap_calculator.py:1054-1810), on the device.
+
+    By default the calculator sees every scene it is to score: with data parallelism the caller gathers the batches
+    first (the reference's `all_gather_dict`).  `world_size > 1` makes it rank-local, for a data-parallel loop that
+    feeds each rank only its own 1/W of every step: scenes are numbered as the gathered stream would number them
+    (rank r's scene b of a step is scene (scenes before the step on all ranks) + r * B + b), and `compute_metrics()`
+    becomes a collective over `group` that exchanges the ranks' detection records and returns the same dict on every
+    rank."""
 
     def __init__(self, dataset_config, ap_iou_thresh=[0.25, 0.5], class2type_map=None, exact_eval=True, args=None,
-                 ap_config_dict=None, reset_nms_iou=None):
+                 ap_config_dict=None, reset_nms_iou=None, *, rank=0, world_size=1, group=None):
         self.ap_iou_thresh = ap_iou_thresh
         if ap_config_dict is None:
             ap_config_dict = get_ap_config_dict(dataset_config=dataset_config, remove_empty_box=exact_eval)
@@ -210,12 +347,16 @@ class APCalculator(object):
         self.args = args
         self.dataset_config = dataset_config
         self.reset_nms_iou = reset_nms_iou
+        if not 0 <= rank < world_size:
+            raise ValueError(f"rank {rank} outside a world of {world_size}")
+        self.rank, self.world_size, self.group = rank, world_size, group
         self.reset()
 
     def reset(self):
         self._scores = []          # per step: (B, K, C) f32, -inf = no detection
         self._live = []            # per step: (B, K) bool
         self._tp = []              # per step: (T, B, C, K) bool
+        self._scene_base = []      # per step: global number of the step's first scene on this rank
         self._gt_count = None      # (C,) int64 ground-truth boxes per class
         # first appearance of every class among the predictions / the ground truth, in the order the reference's
         # dictionaries are filled (utils/eval_det.py:185-207): its group means (mAP_fre = the first four entries ...)
@@ -259,7 +400,9 @@ class APCalculator(object):
         # proposals, box by box otherwise -- then the ground truth scene by scene, box by box
         b, k = det_mask.shape
         big = torch.iinfo(torch.int64).max
-        scene = (self.scan_cnt + torch.arange(b, device=scores.device)).view(b, 1, 1)
+        base = self.scan_cnt + self.rank * b
+        self._scene_base.append(base)
+        scene = (base + torch.arange(b, device=scores.device)).view(b, 1, 1)
         is_det = det_mask.unsqueeze(-1) & torch.isfinite(scores)                       # (B, K, C)
         if cfg["per_class_proposal"]:
             pos = (scene * ncls + torch.arange(ncls, device=scores.device).view(1, 1, ncls)) * k \
@@ -268,59 +411,90 @@ class APCalculator(object):
             pos = (scene * k + torch.arange(k, device=scores.device).view(1, k, 1)).expand(b, k, ncls)
         first_pred = torch.where(is_det, pos.expand(b, k, ncls), torch.full_like(pos.expand(b, k, ncls), big)).amin(dim=(0, 1))
         g = gcls.shape[1]
-        gpos = (self.scan_cnt + torch.arange(b, device=scores.device)).view(b, 1) * g + torch.arange(g, device=scores.device)
+        gpos = (base + torch.arange(b, device=scores.device)).view(b, 1) * g + torch.arange(g, device=scores.device)
         first_gt = torch.full((ncls,), big, dtype=torch.int64, device=scores.device)
         first_gt.scatter_reduce_(0, gcls.clamp(0, ncls - 1)[present], gpos[present], reduce="amin")
         self._first_pred = first_pred if self._first_pred is None else torch.minimum(self._first_pred, first_pred)
         self._first_gt = first_gt if self._first_gt is None else torch.minimum(self._first_gt, first_gt)
-        self.scan_cnt += scores.shape[0]
+        self.scan_cnt += self.world_size * b
 
     # ------------------------------------------------------------------ metrics
-    def _per_class(self):
-        """-> (score, tp[T]) arrays per class with at least one detection, ground-truth counts, class list"""
-        scores = torch.cat([s.reshape(-1, s.shape[-1]) for s in self._scores])            # (N, C)
-        live = torch.cat([m.reshape(-1) for m in self._live])                              # (N,)
-        tps = torch.cat([t.permute(0, 1, 3, 2).reshape(t.shape[0], -1, t.shape[2]) for t in self._tp], dim=1)  # (T, N, C)
-        is_det = live.unsqueeze(-1) & torch.isfinite(scores)
-        npos = self._gt_count.cpu().numpy()
-        out = {}
-        has_det = is_det.any(dim=0).cpu().numpy()
-        for c in range(scores.shape[1]):
-            if not has_det[c] and npos[c] == 0:
-                continue            # the reference only evaluates classes that occur in predictions or ground truth
-            sel = is_det[:, c]
-            s = scores[sel, c]
-            order = torch.argsort(-s, stable=True)
-            out[c] = (s[order].cpu().numpy().astype(np.float64),
-                      tps[:, sel, c][:, order].cpu().numpy().astype(np.float64))
-        return out, npos
+    def rank_state(self) -> RankState:
+        """This calculator's accumulation as detection records and per-class totals (nothing gathered)."""
+        if not self._scores:
+            return RankState(None, None, None, None, [])
+        rec = eval_records(self._scores, self._live, self._tp, self._scene_base)
+        return RankState(rec, self._gt_count, self._first_pred, self._first_gt, [s.shape[0] for s in self._scores])
 
-    def _class_order(self, classes):
+    def _all_rank_state(self, mine: RankState) -> RankState:
+        """The collective behind a rank-local compute_metrics(): every rank ends with the merged state."""
+        import torch.distributed as dist
+
+        w, grp = self.world_size, self.group
+        # gloo exchanges host tensors, NCCL device tensors; the merged state is reduced on this rank's device
+        dev = torch.device("cpu") if dist.get_backend(grp) == "gloo" else torch.device("cuda", torch.cuda.current_device())
+
+        def gather(t):
+            parts = [torch.empty_like(t) for _ in range(w)]
+            dist.all_gather(parts, t, group=grp)
+            return parts
+
+        nsteps = [int(x) for x in gather(torch.tensor([len(mine.batch_sizes)], dtype=torch.int64, device=dev))]
+        if len(set(nsteps)) != 1:
+            raise ValueError(f"data-parallel evaluation needs the same number of steps on every rank, got {nsteps}")
+        if nsteps[0] == 0:
+            return mine
+        sizes = gather(torch.tensor(mine.batch_sizes, dtype=torch.int64, device=dev))
+        _check_batch_sizes([s.tolist() for s in sizes])
+        home = mine.gt_count.device
+        counts = [int(x) for x in gather(torch.tensor([len(mine.records)], dtype=torch.int64, device=dev))]
+        packed = torch.zeros((max(counts), 5), dtype=torch.int32, device=dev)
+        packed[:counts[dist.get_rank(grp)]] = pack_records(mine.records).to(dev)
+        records = merge_records([unpack_records(p[:n].to(home)) for p, n in zip(gather(packed), counts)])
+        totals = []
+        for t, op in ((mine.gt_count, dist.ReduceOp.SUM), (mine.first_pred, dist.ReduceOp.MIN),
+                      (mine.first_gt, dist.ReduceOp.MIN)):
+            t = t.to(dev, copy=True)
+            dist.all_reduce(t, op=op, group=grp)
+            totals.append(t.to(home))
+        return RankState(records, *totals, list(mine.batch_sizes))
+
+    def _class_order(self, classes, first_pred, first_gt):
         """classes in the order the reference's result dictionaries hold them: those that occur among the predictions
         by first occurrence, then the ground-truth-only ones by first occurrence."""
-        fp, fg = self._first_pred.cpu().numpy(), self._first_gt.cpu().numpy()
+        fp, fg = first_pred.cpu().numpy(), first_gt.cpu().numpy()
         big = np.iinfo(np.int64).max
         return sorted(classes, key=lambda c: (0, fp[c]) if fp[c] < big else (1, fg[c]))
 
     def compute_metrics(self):
         """Same dict as the reference (:1531-1703): per IoU threshold the per-class AP / Prec / Recall and the
-        frequency-group means."""
-        per_class, npos = self._per_class() if self._scores else ({}, np.zeros(0))
+        frequency-group means.  In rank-local mode a collective: every rank must call it, and every rank gets the
+        metrics of all ranks' scenes."""
+        state = self.rank_state()
+        if self.world_size > 1:
+            state = self._all_rank_state(state)
+        return self.metrics_from_state(state)
+
+    def metrics_from_state(self, state: RankState):
+        """compute_metrics() on an accumulated state (`rank_state()`, or `merge_rank_states` of several)."""
+        nthr = len(self.ap_iou_thresh)
+        if state.gt_count is None:
+            classes, ap, last_prec, last_rec, nrec = [], None, None, None, None
+        else:
+            ncls = state.gt_count.shape[0]
+            ap, last_prec, last_rec, counts, _ = eval_ap(sort_records(state.records), ncls, nthr, state.gt_count)
+            ap, last_prec, last_rec, nrec, npos = (x.cpu().numpy() for x in (ap, last_prec, last_rec, counts,
+                                                                              state.gt_count))
+            # the reference only evaluates classes that occur in predictions or ground truth
+            classes = [c for c in range(ncls) if nrec[c] > 0 or npos[c] > 0]
+        ordered = self._class_order(classes, state.first_pred, state.first_gt) if classes else []
+        name = lambda key: self.class2type_map[key] if self.class2type_map else str(key)  # noqa: E731
         overall_ret = OrderedDict()
         for ti, thresh in enumerate(self.ap_iou_thresh):
-            rec, prec, ap = {}, {}, {}
-            for c, (_, tp_all) in per_class.items():
-                tp = np.cumsum(tp_all[ti])
-                fp = np.cumsum(1.0 - tp_all[ti])
-                rec[c] = np.zeros_like(tp) if npos[c] == 0 else tp / float(npos[c])
-                prec[c] = tp / np.maximum(tp + fp, np.finfo(np.float64).eps)
-                ap[c] = voc_ap(rec[c], prec[c])
             ret_dict = OrderedDict()
-            name = lambda key: self.class2type_map[key] if self.class2type_map else str(key)  # noqa: E731
-            for key in sorted(ap.keys()):
-                ret_dict["%s Average Precision" % name(key)] = ap[key]
-            ordered = self._class_order(list(ap.keys())) if ap else []
-            ap_vals = np.array([ap[key] for key in ordered], dtype=np.float32)
+            for key in classes:
+                ret_dict["%s Average Precision" % name(key)] = np.float64(ap[ti, key])
+            ap_vals = np.array([ap[ti, key] for key in ordered], dtype=np.float32)
             ap_vals[np.isnan(ap_vals)] = 0
             scannet = (getattr(self.args, "dataset_name", "") or "").find("scannet") != -1 and ap_vals.shape[0] >= 21
 
@@ -341,14 +515,15 @@ class APCalculator(object):
 
             ret_dict["mAP"] = ap_vals.mean() if ap_vals.size else 0.0
             groups("mAP", ap_vals)
+            # per-class entries are emitted by sorted key (:1605-1623), so the LISTS behind the group means are sorted;
+            # a class with ground truth but no detection has an empty curve, whose last value the reference reads as 0
             prec_list, rec_list = [], []
-            # per-class entries are emitted by sorted key (:1605-1623), so the LISTS behind the group means are sorted
-            for key in sorted(prec.keys()):
-                last = prec[key][-1] if len(prec[key]) else 0
+            for key in classes:
+                last = np.float64(last_prec[ti, key]) if nrec[key] else 0
                 ret_dict["%s Prec" % name(key)] = last
                 prec_list.append(last)
-            for key in sorted(ap.keys()):
-                last = rec[key][-1] if len(rec[key]) else 0
+            for key in classes:
+                last = np.float64(last_rec[ti, key]) if nrec[key] else 0
                 ret_dict["%s Recall" % name(key)] = last
                 rec_list.append(last)
             groups("Prec", prec_list)

@@ -58,6 +58,38 @@ int coda_eval_match(int b, int k, int g, int ncls, const float *iou, const float
                     const unsigned char *det_mask, const int *gt_cls, const unsigned char *gt_present, float iou_thresh,
                     unsigned char *tp, void *stream);
 
+/*
+ * Detection records of one accumulated step, appended through a device counter:
+ *   for every (scene bb, box j, class c) with det_mask (b, k) uint8 set and scores (b, k, ncls) fp32 finite (-inf
+ *   marks "no detection of class c", NaN is no detection either) one record at slot atomicAdd(counter, 1):
+ *     rec_cls   int32  c
+ *     rec_score fp32   scores[bb, j, c] (-0 written as +0)
+ *     rec_pos   int64  (scene_base + bb) * k + j    -- the global (scene, box) position that breaks score ties
+ *     rec_tp    uint32 bit t = tp[t, bb, c, j] != 0, tp (nthr, b, ncls, k) uint8, 1 <= nthr <= 32
+ *   Slots are taken in no particular order.  Slots at or past `capacity` are not written; the counter still counts
+ *   them, so a counter above the capacity after the launch means the buffers were too small.  The caller zeroes the
+ *   counter before the first step and may append several steps (each with its own scene_base) to one buffer.
+ */
+int coda_eval_records(int b, int k, int ncls, int nthr, long long scene_base, const float *scores,
+                      const unsigned char *det_mask, const unsigned char *tp, int *counter, int capacity,
+                      int *rec_cls, float *rec_score, long long *rec_pos, unsigned *rec_tp, void *stream);
+
+/*
+ * Precision / recall / VOC AP of every (class, IoU threshold) in one launch (utils/eval_det.py:147-162 and voc_ap
+ * with use_07_metric=False, :23-55), all in fp64.
+ *   rec_tp (nrec) uint32: the true-positive masks of the records sorted by (class ascending, score descending, global
+ *   position ascending); offsets (ncls + 1) int64: class c owns records [offsets[c], offsets[c + 1]); npos (ncls)
+ *   int64: ground-truth boxes per class.  For record i of a segment, with cum_i its true positives up to i:
+ *     precision_i = cum_i / max(i + 1, eps), recall_i = cum_i / npos (0 where npos == 0), the envelope
+ *     max_{j >= i} precision_j, AP = sum of (recall_i - recall_{i-1}) * envelope_i where the recall steps.
+ *   ap, last_prec, last_rec (nthr, ncls) fp64; a class without records gets 0, 0, 0.  curves, if not NULL,
+ *   (nthr, 4, nrec) fp64 receives per record the cumulative TP, cumulative FP, recall and precision.
+ *   Counts, precision and recall are exactly numpy's; the AP sum is taken in another order.
+ */
+int coda_eval_ap(int ncls, int nthr, long long nrec, const long long *offsets, const unsigned *rec_tp,
+                 const long long *npos, double *ap, double *last_prec, double *last_rec, double *curves,
+                 void *stream);
+
 #ifdef __cplusplus
 }
 #endif
