@@ -114,34 +114,37 @@ def scannet_prompt_class_ids(train_ids, test_ids, reset_num: int) -> list:
     return sorted(ids)
 
 
-def _scannet_class_names(args):
+def _scannet_class_names(args, evaluated: bool):
     if not (os.path.exists(SCANNET_CLASS_NAMES_PATH) and os.path.exists(SCANNET_CLASS_IDS_PATH)):
         return None
     names = np.load(SCANNET_CLASS_NAMES_PATH)
     rows = scannet_class_rows(names, np.load(SCANNET_CLASS_IDS_PATH, allow_pickle=True).item())
     train = [int(i) for i in args.train_range_list]
-    if getattr(args, "if_clip_more_prompts", False):
+    if evaluated:
         ids = scannet_prompt_class_ids(train, [int(i) for i in args.test_range_list], int(args.reset_scannet_num))
     else:
         ids = train                                  # the seen classes, in the order given
     return [names[rows[i]] for i in ids]
 
 
-def _class_prompts(args):
-    """'a photo of a {class} in the scene' prompts of the seen / evaluated classes
-    (reference :197-279).  Needs the class lists of a CoDA checkout (relative paths, as
+def _class_prompts(args, evaluated=None):
+    """'a photo of a {class} in the scene' prompts of the seen (`evaluated` False) or evaluated classes (None: as
+    --if_clip_more_prompts says)
+    (reference :197-279, :1923-1988).  Needs the class lists of a CoDA checkout (relative paths, as
     in the reference); returns None when they are not reachable (synthetic runs).
     SUN RGB-D: the first train_range_max / test_range_max names of the class dictionary.
     ScanNet (dataset_name contains "scannet"): the ScanNet-200 names picked by class id through
     train_range_list / test_range_list / reset_scannet_num."""
+    if evaluated is None:
+        evaluated = getattr(args, "if_clip_more_prompts", False)
     if getattr(args, "dataset_name", "").find("scannet") != -1:
-        names = _scannet_class_names(args)
+        names = _scannet_class_names(args, evaluated)
         return None if names is None else [_prompt(c) for c in names]
     path = ALL_CLASS_PATH_V1 if getattr(args, "if_use_v1", True) else ALL_CLASS_PATH_V2
     if not os.path.exists(path):
         return None
     names = list(np.load(path, allow_pickle=True).item().keys())
-    n = args.test_range_max if getattr(args, "if_clip_more_prompts", False) else args.train_range_max
+    n = args.test_range_max if evaluated else args.train_range_max
     return [_prompt(c) for c in names[:n]]
 
 
@@ -156,7 +159,7 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
                  if_with_fake_classes=False, pooling_methods="average", if_clip_more_prompts=False,
                  if_keep_box=False, if_select_box_by_objectness=False, keep_objectness=0.5,
                  online_nms_update_novel_label=False, online_nms_update_accumulate_novel_label=False,
-                 online_nms_update_accumulate_epoch=10, distillation_box_num=32, args=None):
+                 online_nms_update_accumulate_epoch=10, distillation_box_num=32, args=None, has_clip=None):
         super().__init__()
         self.if_with_fake_classes = if_with_fake_classes
         self.num_cls_predict = num_cls_predict
@@ -166,6 +169,7 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
         self.if_with_clip = if_with_clip
         self.if_clip_more_prompts = if_clip_more_prompts
         self.if_with_clip_train = if_with_clip_train
+        self.has_clip = if_with_clip_train if has_clip is None else has_clip     # a frozen CLIP and the text features
         self.box_idx_list = np.arange(128, dtype=np.int8)  # reference :191 (fixed, whatever nqueries is)
         self.external_selection = None  # device (B, 32) int64 tensor when the step is CUDA-graph captured
         self.if_keep_box = if_keep_box
@@ -176,14 +180,13 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
         self.test_range_max = args.test_range_max
         self.if_clip_superset = getattr(args, "if_clip_superset", False)
 
-        if self.if_with_clip_train:
+        if self.has_clip:
             self._build_clip(args, dataset_config)
 
-        # NB the reference hard-codes input_dim=256, hidden [512, 512] here (:409-412)
         self.encoder_to_decoder_projection = GenericMLP(
-            input_dim=256, hidden_dims=[512, 512], output_dim=decoder_dim, norm_fn_name="bn1d",
-            activation="relu", use_conv=True, output_use_activation=True, output_use_norm=True,
-            output_use_bias=False)
+            input_dim=self._projection_dims(encoder_dim)[0], hidden_dims=self._projection_dims(encoder_dim)[1],
+            output_dim=decoder_dim, norm_fn_name="bn1d", activation="relu", use_conv=True,
+            output_use_activation=True, output_use_norm=True, output_use_bias=False)
         self.pos_embedding = PositionEmbeddingCoordsSine(d_pos=decoder_dim, pos_type=position_embedding,
                                                          normalize=True)
         self.query_projection = GenericMLP(
@@ -208,7 +211,20 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
         self.if_accumulate_former_pseudo_labels = getattr(args, "if_accumulate_former_pseudo_labels", False)
         self._pending_pseudo = None
 
+    def _projection_dims(self, encoder_dim):
+        """(input_dim, hidden_dims) of encoder_to_decoder_projection: the reference hard-codes 256, [512, 512] in
+        this head (:409-412)."""
+        return 256, [512, 512]
+
     # ------------------------------------------------------------------ CLIP side
+    # True: the prompts of the evaluated classes (test_range_max); False: the seen ones (train_range_max).  The CoDA
+    # head follows --if_clip_more_prompts
+    def _evaluated_prompts(self, args):
+        return getattr(args, "if_clip_more_prompts", False)
+
+    # True: normalise the text features in CLIP's own dtype (fp16 on the GPU), then cast to fp32
+    TEXT_NORM_IN_CLIP_DTYPE = False
+
     def _build_clip(self, args, dataset_config):
         """Frozen CLIP + L2-normalised text features of the class prompts (reference :197-399).
         The reference loads the same checkpoint twice (`clip_model`, `test_clip_model`);
@@ -226,7 +242,8 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
         res = self.clip_model.visual.input_resolution
         self.clip_resolution = res
 
-        prompts = _class_prompts(args)
+        evaluated = self._evaluated_prompts(args)
+        prompts = _class_prompts(args, evaluated)
         tokens = None
         if prompts is not None:
             try:
@@ -240,7 +257,8 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
         self.all_classes_keys = prompts
         with torch.no_grad():
             if tokens is not None:
-                feats = self.clip_model.encode_text(tokens).to(torch.float32)
+                raw = self.clip_model.encode_text(tokens)
+                feats = raw.to(torch.float32)
             else:
                 # synthetic run: random unit rows stand in for the text embeddings (SURVEY.md 8d)
                 if os.path.exists(ckpt):
@@ -248,11 +266,12 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
                                        "the text features would be meaningless")
                 warnings.warn("class prompts unavailable: RANDOM unit rows stand in for the CLIP text features "
                               "(throughput / parity runs only; class scores and weak labels are meaningless)")
-                n = args.test_range_max if self.if_clip_more_prompts else args.train_range_max
+                n = args.test_range_max if evaluated else args.train_range_max
                 g = torch.Generator().manual_seed(1234)
-                feats = torch.randn(n, self.clip_model.visual.output_dim, generator=g).to(self.device)
+                feats = raw = torch.randn(n, self.clip_model.visual.output_dim, generator=g).to(self.device)
             self.text_features_fg = feats
-            self.text_features_fg_norm = (feats / feats.norm(dim=1, keepdim=True)).to(torch.float32)
+            src = raw if self.TEXT_NORM_IN_CLIP_DTYPE else feats
+            self.text_features_fg_norm = (src / src.norm(dim=1, keepdim=True)).to(torch.float32)
             if self.if_clip_superset:
                 nsup = getattr(args, "superset_size", 1201)
                 g = torch.Generator().manual_seed(4321)
@@ -268,10 +287,10 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
         self.to(device)
         self.device = str(device)
         for name in ("text_features_fg", "text_features_fg_norm", "superset_text_features_fg_norm",
-                     "test_text_features_fg_norm"):
-            if isinstance(getattr(self, name, None), torch.Tensor):
+                     "test_text_features_fg_norm", "test_logit_scale", "logit_scale"):
+            if isinstance(getattr(self, name, None), torch.Tensor) and name not in self._parameters:
                 setattr(self, name, getattr(self, name).to(device))
-        if str(device) == "cpu" and self.if_with_clip_train:
+        if str(device) == "cpu" and self.has_clip:
             self.clip_model.float()
         return self
 
@@ -330,13 +349,13 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
         # land directly in (num_layers, batch, nqueries, out) order
         rows = box_features.permute(0, 2, 1, 3).reshape(num_layers * batch * num_queries, channel)
         # six heads read the same rows: their six input gradients meet in one n-ary sum (ops.fanout)
-        taps = iter(ops.fanout(rows, 6))
+        taps = iter(ops.fanout(rows, len(self.mlp_heads)))
 
         def head(name):
             return self.mlp_heads[name].forward_rows(next(taps)).view(num_layers, batch, num_queries, -1)
 
         cls_logits = head("sem_cls_head")
-        text_correlation_embedding = head("text_correlation_head")
+        text_correlation_embedding = head("text_correlation_head") if "text_correlation_head" in self.mlp_heads else None
         center_offset = head("center_head").sigmoid() - 0.5
         size_normalized = head("size_head").sigmoid()
         angle_logits = head("angle_cls_head")
@@ -361,7 +380,6 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
         lay = lambda t: t.reshape(num_layers, batch, *t.shape[1:])  # noqa: E731
         stacked = {
             "sem_cls_logits": cls_logits,
-            "text_correlation_embedding": text_correlation_embedding,
             "center_normalized": lay(center_normalized.contiguous()),
             "center_unnormalized": lay(center_unnormalized),
             "size_normalized": size_normalized,
@@ -375,6 +393,8 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
             "box_corners": lay(box_corners),
             "box_corners_xyz": lay(box_corners_xyz),
         }
+        if text_correlation_embedding is not None:
+            stacked["text_correlation_embedding"] = text_correlation_embedding
         outputs = []
         for l in range(num_layers):   # the reference's per-layer dicts are views into the stacked tensors
             d = {k: v[l] for k, v in stacked.items()}
@@ -435,19 +455,25 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
             vd = vd & chosen
         vd = vd.reshape(-1)
         scene = torch.arange(bsz, device=boxes.device, dtype=torch.int32).repeat_interleave(nsel)
+        feats = self._encode_crops(inputs["input_image"], scene, bx, vd)
+        return feats.reshape(bsz, nsel, -1), vd.reshape(bsz, nsel)
+
+    @torch.no_grad()
+    def _encode_crops(self, images, scene, boxes, valid):
+        """CLIP image features (N, D) fp32 of the crops boxes (N, 4) of images[scene] (garbage where not valid)."""
         extra = {}
         visual = getattr(self.clip_model, "visual", None)
-        if (inputs["input_image"].is_cuda and self.clip_model.dtype == torch.float16
+        if (images.is_cuda and self.clip_model.dtype == torch.float16
                 and isinstance(visual, clip_mod.model.VisionTransformer)):
             ps = visual.conv1.kernel_size[0]
             if self.clip_resolution % ps == 0 and (3 * ps * ps) % 64 == 0:
                 extra["patch"] = ps        # crops come out as the unfolded patches the ViT's first GEMM reads
-        crops = ops.crop_resize_normalize(inputs["input_image"], scene, bx, vd, self.clip_resolution,
+        crops = ops.crop_resize_normalize(images, scene, boxes, valid, self.clip_resolution,
                                           dtype=self.clip_model.dtype, **extra)
         feats = self.clip_model.encode_image(crops)
         if isinstance(feats, tuple):
             feats = feats[0]
-        return feats.to(torch.float32).reshape(bsz, nsel, -1), vd.reshape(bsz, nsel)
+        return feats.to(torch.float32)
 
     @torch.no_grad()
     def get_predicted_box_clip_embedding(self, inputs, outputs, thres_obj=0.05, if_use_gt_box=False,
@@ -654,6 +680,11 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
         tgt = torch.zeros_like(query_embed, memory_format=torch.contiguous_format)
         box_features = self.decoder(tgt, enc_features, query_pos=query_embed, pos=enc_pos)[0]
         box_predictions = self.get_box_predictions(query_xyz, point_cloud_dims, box_features, point_clouds, inputs)
+        return self._clip_outputs(inputs, box_predictions, if_test, if_real_test, if_cmp_class, curr_epoch)
+
+    def _clip_outputs(self, inputs, box_predictions, if_test, if_real_test, if_cmp_class, curr_epoch):
+        """The CLIP side of forward (reference :1776-1831): distillation targets in training, class scores at test."""
+        point_clouds = inputs["point_clouds"]
         out = box_predictions["outputs"]
         if self.if_with_clip_train:
             out["logit_scale"] = torch.clip(self.logit_scale.exp(), min=None, max=100)
@@ -675,6 +706,170 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
             out["text_features_clip"] = self.text_features_fg_norm.unsqueeze(0).repeat(point_clouds.shape[0], 1, 1)
             box_predictions, _, _ = self.get_class_scores(box_predictions)
         return box_predictions
+
+
+def read_scannet_matrix(path) -> np.ndarray:
+    """The 4 x 4 matrix of a ScanNet calibration text file (intrinsic/intrinsic_color.txt, pose/<frame>.txt): 16
+    numbers, row by row, as the reference's load_txt reads them (datasets/scannet_utils.py:69-79)."""
+    path = str(path)
+    if not os.path.isfile(path):
+        raise FileNotFoundError(f"ScanNet calibration file not found: {path}")
+    with open(path) as f:
+        vals = [float(x) for x in f.read().split()]
+    if len(vals) != 16:
+        raise ValueError(f"{path}: expected the 16 numbers of a 4 x 4 matrix, found {len(vals)}")
+    return np.array(vals, dtype=np.float64).reshape(4, 4)
+
+
+class ScanNetCalibration:
+    """The colour intrinsics and camera-to-world poses of ScanNet scenes, read from `<calib_name>/intrinsic/
+    intrinsic_color.txt` and `<calib_name>/pose/<squence_name>.txt` as the reference's SCANNET_Calibration does
+    (datasets/scannet_utils.py:110-130); each file is read once."""
+
+    def __init__(self):
+        self._cache = {}
+
+    def matrix(self, path) -> np.ndarray:
+        path = str(path)
+        if path not in self._cache:
+            self._cache[path] = read_scannet_matrix(path)
+        return self._cache[path]
+
+    def __call__(self, calib_names, squence_names):
+        """-> (K (B, 4, 4), pose (B, 4, 4)) fp64 host arrays for the scenes of a batch."""
+        K = [self.matrix(os.path.join(str(c), "intrinsic", "intrinsic_color.txt")) for c in calib_names]
+        pose = [self.matrix(os.path.join(str(c), "pose", f"{s}.txt")) for c, s in zip(calib_names, squence_names)]
+        return np.stack(K), np.stack(pose)
+
+
+class Model3DETRMultiClassHead(Model3DETRPredictedBoxDistillationHead):
+    """The 3DETR + CLIP baseline of the paper (reference Model3DETRMultiClassHead, :1838-3932): the 3DETR heads
+    with a class-agnostic objectness head and no text-correlation head, and a frozen CLIP that classifies every
+    predicted box by its image crop at test time (`forward(if_real_test=True)`, reference clip_to_class_training
+    :2810-3085).  Training never crops."""
+
+    # crops per CLIP tower call at test time: bounds the tower's activations (the ViT-B/16 MLP hidden activation alone
+    # is 1.2 MB per crop in fp16) whatever the batch size
+    CROPS_PER_CALL = 1024
+    TEXT_NORM_IN_CLIP_DTYPE = True          # reference :2088-2090: fp16 features normalised in fp16, then fp32
+
+    def __init__(self, pre_encoder, encoder, decoder, dataset_config, encoder_dim=256, decoder_dim=256,
+                 position_embedding="fourier", mlp_dropout=0.3, num_queries=256, if_use_gt_box=False,
+                 if_expand_box=False, args=None):
+        for flag, on in (("if_use_gt_box", if_use_gt_box), ("if_expand_box", if_expand_box),
+                         ("if_only_novel_prompt", getattr(args, "if_only_novel_prompt", False)),
+                         ("online_nms_update_save_novel_label_clip_driven_with_cate_confidence",
+                          getattr(args, "online_nms_update_save_novel_label_clip_driven_with_cate_confidence", False))):
+            if on:
+                raise NotImplementedError(f"the baseline head does not implement --{flag}")
+        self._masked_encoder = hasattr(encoder, "masking_radius")
+        super().__init__(pre_encoder, encoder, decoder, dataset_config, encoder_dim=encoder_dim,
+                         decoder_dim=decoder_dim, position_embedding=position_embedding, mlp_dropout=mlp_dropout,
+                         num_queries=num_queries, if_with_clip_train=False, num_cls_predict=1, args=args,
+                         has_clip=True)
+        # reference :2082: a plain tensor (not a parameter, so no state-dict entry), used unclipped at test time
+        del self.logit_scale
+        self.logit_scale = self.test_logit_scale
+        # the reference's baseline holds CLIP once, as clip_model: no aliases, so that its checkpoints load strictly
+        del self.test_clip_model, self.res_encoder
+        self.scannet_calibration = ScanNetCalibration()
+
+    def _projection_dims(self, encoder_dim):
+        # reference :1886-1900
+        return encoder_dim, ([encoder_dim] if self._masked_encoder else [encoder_dim, encoder_dim])
+
+    def _evaluated_prompts(self, args):
+        return True                          # reference :1923-1988: always the test_range_max / evaluated classes
+
+    def build_mlp_heads(self, dataset_config, decoder_dim, mlp_dropout):
+        # reference :2145-2176: objectness (1 + 1 logits) and the box geometry
+        mlp_func = partial(GenericMLP, norm_fn_name="bn1d", activation="relu", use_conv=True,
+                           hidden_dims=[decoder_dim, decoder_dim], dropout=mlp_dropout, input_dim=decoder_dim)
+        self.mlp_heads = nn.ModuleDict([
+            ("sem_cls_head", mlp_func(output_dim=1 + 1)),
+            ("center_head", mlp_func(output_dim=3)),
+            ("size_head", mlp_func(output_dim=3)),
+            ("angle_cls_head", mlp_func(output_dim=dataset_config.num_angle_bin)),
+            ("angle_residual_head", mlp_func(output_dim=dataset_config.num_angle_bin)),
+        ])
+
+    def _clip_outputs(self, inputs, box_predictions, if_test, if_real_test, if_cmp_class, curr_epoch):
+        # reference :3903-3926
+        if if_cmp_class:
+            raise NotImplementedError("the baseline head does not implement if_cmp_class")
+        out = box_predictions["outputs"]
+        out["logit_scale"] = torch.clip(self.logit_scale.exp(), min=None, max=100)
+        if not (if_real_test or if_test):
+            text = (self.superset_text_features_fg_norm if self.if_clip_superset
+                    else self.text_features_fg_norm[: self.train_range_max, :])
+            out["text_features_clip"] = text.unsqueeze(0).repeat(inputs["point_clouds"].shape[0], 1, 1)
+        if if_real_test:
+            self.classify_boxes(inputs, out)
+        return box_predictions
+
+    def _camera_inputs(self, inputs, bsz: int, dev):
+        """The batch's camera with identity augmentation: the reference's test path projects the predicted boxes
+        with the scene's calibration alone (:2905-2938).  ScanNet test batches carry no K / Rtilt: their
+        calibration files are read (reference SCANNET_Calibration)."""
+        if "K" in inputs and "Rtilt" in inputs:
+            K, Rtilt = inputs["K"], inputs["Rtilt"]
+        elif self.dataset_name == "scannet":
+            K, Rtilt = (torch.from_numpy(a).to(dev) for a in
+                        self.scannet_calibration(inputs["calib_name"], inputs["squence_name"]))
+        else:
+            raise KeyError("the baseline head's test-time classification needs the batch's K and Rtilt")
+        f64 = dict(device=dev, dtype=torch.double)
+        # the test path clamps the projected extent to [0, width] x [0, height] (:2935-2938) where the training path,
+        # which the kernel follows, clamps to [0, width - 1] x [0, height - 1]
+        cam = {k: inputs[k] + 1 for k in ("ori_width", "ori_height")}
+        cam.update({k: inputs[k] for k in ("x_offset", "y_offset")})
+        cam.update(K=K, Rtilt=Rtilt, scale_array=torch.ones((bsz, 1, 3), **f64),
+                   rot_array=torch.eye(3, **f64).expand(bsz, 3, 3), flip_array=torch.ones((bsz, 1), **f64),
+                   image_flip_array=torch.ones((bsz, 1), **f64), flip_length=torch.zeros((bsz,), **f64))
+        return cam
+
+    @torch.no_grad()
+    def project_boxes(self, inputs, out, extent=False):
+        """ops.boxes_in_image of every predicted box as the reference's test path projects it: the scene's
+        calibration, no augmentation, the dataset's camera."""
+        bsz = out["box_corners_xyz"].shape[0]
+        corners, camera = out["box_corners_xyz"], {}
+        if self.dataset_name == "scannet":
+            camera = {"camera": "scannet"}
+            # the ScanNet test path turns the box by +angle (datasets/scannet_utils.py:402, rotz(box_angle)); the
+            # corner builder, like SUN RGB-D's projection (sunrgbd_utils.py:364), turns it by -angle
+            corners = self.box_processor.box_parametrization_to_corners_xyz(
+                out["center_unnormalized"], out["size_unnormalized"], -out["angle_continuous"])
+        return ops.boxes_in_image(corners, out["size_unnormalized"],
+                                  self._camera_inputs(inputs, bsz, corners.device), extent=extent, **camera)
+
+    @torch.no_grad()
+    def classify_boxes(self, inputs, out):
+        """out['sem_cls_prob'] (B, Q, test_range_max) = softmax(logit_scale * f_hat . text^T) of the CLIP feature f of
+        each box's crop, zeros for a box without a usable crop; out['sem_cls_logits'] zeros (reference :2810-3085).
+        The usable boxes are compacted on the device (one read of their count per batch) and only their crops go
+        through the tower, CROPS_PER_CALL at a time."""
+        bsz, nq = out["box_corners_xyz"].shape[:2]
+        dev = out["box_corners_xyz"].device
+        boxes, valid = self.project_boxes(inputs, out)
+        idx = valid.reshape(-1).nonzero().squeeze(1)
+        n = idx.numel()
+        row_map = torch.full((bsz * nq,), -1, dtype=torch.int32, device=dev)
+        row_map[idx] = torch.arange(n, dtype=torch.int32, device=dev)
+        text = self.text_features_fg_norm
+        feats = torch.empty((n, text.shape[1]), dtype=torch.float32, device=dev)
+        flat_boxes = boxes.reshape(-1, 4)
+        for s in range(0, n, self.CROPS_PER_CALL):
+            sel = idx[s: s + self.CROPS_PER_CALL]
+            scene = torch.div(sel, nq, rounding_mode="floor").to(torch.int32)
+            feats[s: s + sel.numel()] = self._encode_crops(inputs["input_image"], scene, flat_boxes[sel],
+                                                          torch.ones_like(sel, dtype=torch.bool))
+        out["sem_cls_prob"], out["sem_cls_logits"] = ops.clip_classify(feats, text, self.logit_scale, row_map,
+                                                                       (bsz, nq))
+        out["clip_usable_mask"] = valid
+        out["clip_boxes_2d"] = boxes
+        out["clip_crop_features"] = feats
+        return out
 
 
 def build_preencoder(args):
@@ -722,11 +917,10 @@ def build_3detr_predictedbox_distillation_head(args, dataset_config):
 
 
 def build_3detr_multiclasshead(args, dataset_config):
-    """The plain 3DETR baseline head (reference Model3DETRMultiClassHead, :1838): same
-    geometry path without the CLIP alignment branch."""
+    """The 3DETR + CLIP baseline head (reference Model3DETRMultiClassHead, :1838-3932, built as :4052-4072)."""
     g = lambda name, default=False: getattr(args, name, default)  # noqa: E731
-    model = Model3DETRPredictedBoxDistillationHead(
+    model = Model3DETRMultiClassHead(
         build_preencoder(args), build_encoder(args), build_decoder(args), dataset_config,
         encoder_dim=args.enc_dim, decoder_dim=args.dec_dim, mlp_dropout=args.mlp_dropout,
-        num_queries=args.nqueries, if_with_clip_train=False, num_cls_predict=dataset_config.num_semcls, args=args)
+        num_queries=args.nqueries, if_use_gt_box=g("if_use_gt_box"), if_expand_box=g("if_expand_box"), args=args)
     return model, BoxProcessor(dataset_config)

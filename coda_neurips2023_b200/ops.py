@@ -860,6 +860,33 @@ def crop_resize_normalize(images: torch.Tensor, scene: torch.Tensor, boxes: torc
     return out
 
 
+@torch.no_grad()
+def clip_classify(feats: torch.Tensor, text: torch.Tensor, scale: torch.Tensor, row_map: torch.Tensor,
+                  shape) -> tuple:
+    """Class probabilities of every (scene, query) row from its crop's CLIP feature (include/coda_image.h
+    coda_clip_classify).  feats (n, 512) fp32 of the compacted crops, text (C, 512) normalised fp32, scale a
+    one-element device tensor, row_map (B * Q) int32 (-1 = no crop) -> (sem_cls_prob (*shape, C): softmax of
+    scale * f_hat . text^T, zeros where skipped; sem_cls_logits (*shape, C): zeros).  No host synchronisation."""
+    _need_cuda(text, "clip_classify")
+    for name, t in (("feats", feats), ("scale", scale), ("row_map", row_map)):
+        if t.device != text.device:
+            raise ValueError(f"clip_classify: {name} is on {t.device}, the text features on {text.device}")
+    fc, tc, sc = _f32c(feats), _f32c(text), _f32c(scale.reshape(1))
+    rm = row_map.to(torch.int32).contiguous()
+    c, d = tc.shape
+    if fc.shape[1:] != (d,):
+        raise ValueError(f"clip_classify: features of width {tuple(fc.shape[1:])} against text of width {d}")
+    prob = torch.empty((*shape, c), dtype=torch.float32, device=tc.device)
+    logits = torch.empty_like(prob)
+    if prob.numel() // c != rm.numel():
+        raise ValueError(f"clip_classify: {rm.numel()} row-map entries for output rows {tuple(shape)}")
+    with torch.cuda.device(tc.device):
+        st = lib().coda_clip_classify(_ll(rm.numel()), _i(fc.shape[0]), _i(c), _i(d), ptr(fc), ptr(tc), ptr(sc),
+                                      ptr(rm), ptr(prob), ptr(logits), stream_of(tc))
+    check(st, "clip_classify")
+    return prob, logits
+
+
 # --------------------------------------------------------------------------- wgmma GEMM
 # bf16 planes per fp32 operand.  3 -> six cross products, all 24 mantissa bits: fp32-class accuracy, which the
 # 1e-4 parity bar needs through 13 layers (2 planes / 3 products measured 1.4e-4 on the class logits).

@@ -45,6 +45,22 @@ int coda_crop_resize_normalize_ex(int nimg, int h, int w, int ncrops, int res,
                                   int patch, int tile_rows, void *workspace, void *out,
                                   void *stream);
 
+/*
+ * Test-time classification of predicted boxes by their CLIP crops (the baseline head's `if_real_test` path;
+ * replaces the normalise / matmul / softmax / index-put of reference models/model_3detr.py:3056-3064).
+ *   feats    (n, d) fp32    CLIP image features of the n compacted crops
+ *   text     (c, d) fp32    L2-normalised text features of the c class prompts
+ *   scale    (1) fp32, device   the logit scale (read on the device: no host synchronisation)
+ *   row_map  (rows) int32   row of `feats` for each (scene, query) row; -1 (or anything outside [0, n)) = skipped
+ *   prob     (rows, c) fp32  usable rows: softmax(scale * (f / |f|) . text^T); skipped rows: exact zeros
+ *   logits   (rows, c) fp32  written as zeros (the reference leaves sem_cls_logits at zero), may be NULL
+ * The norm, the dot products and the max-subtracted softmax are evaluated in fp64 from the fp32 operands and
+ * rounded once to fp32, in a fixed order: the result is the same bits on every run.  Nothing outside prob and
+ * logits is written; no allocation.  d must be 512 (CODA_EINVAL otherwise); c from 1 to 28000.
+ */
+int coda_clip_classify(long long rows, int n, int c, int d, const float *feats, const float *text,
+                       const float *scale, const int *row_map, float *prob, float *logits, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
