@@ -91,6 +91,9 @@ class SetCriterion(nn.Module):
         self.confidence_type = getattr(args, "confidence_type", "non-confidence")
         assert self.confidence_type in ["non-confidence", "objectness", "clip+objectness", "clip-max-prob"]
         self.if_only_seen_in_loss = getattr(args, "if_only_seen_in_loss", False)
+        # --if_clip_superset: the contrastive loss reads ONE (C, 512) text matrix shared by every scene and layer
+        # (ops.text_contrastive_ce) instead of a per-scene, per-layer copy of it
+        self.if_clip_superset = getattr(args, "if_clip_superset", False)
         # GIoU of rotated boxes: all gt columns (TorchScript reference path) unless the
         # compiled-Cython quirk is requested (see ops / include/coda_detr.h)
         self.giou_rot_k2_limit = 4 if getattr(args, "giou_cython_k2_quirk", False) else None
@@ -208,13 +211,13 @@ class SetCriterion(nn.Module):
         diff = (pred * w - target * w).abs()
         return {"loss_predicted_region_embed_l1": diff.sum(dim=(1, 2, 3)) / ave_weight}
 
+    def _shared_text(self, t: torch.Tensor) -> bool:
+        """True: the contrastive loss of this criterion takes the shared-text path (--if_clip_superset on the GPU)"""
+        return self.if_clip_superset and t.is_cuda
+
     def loss_feat_seen_softmax_weakly_loss_with_novel_cate_confi(self, outputs, targets, assignments):
         """The contrastive loss of stage 2: CE over logit_scale * cos(head embedding, text
         embeddings) with matched (seen) or CLIP-derived (weak) labels (reference :598-644)."""
-        e = outputs["text_correlation_embedding"]
-        e = e / (e.norm(dim=-1, keepdim=True) + 1e-32)
-        text = targets["text_features_clip"].to(torch.float32)
-        corr = torch.bmm(e, text.permute(0, 2, 1)) * targets["logit_scale"]
         inds = assignments["per_prop_gt_inds"]
         matched = assignments["proposal_matched_mask"].int() > 0
         seen_label = torch.gather(targets["gt_box_seen_sem_cls_label"], 1, inds)
@@ -225,8 +228,20 @@ class SetCriterion(nn.Module):
             conf = torch.where(conf > 1e-16, torch.ones_like(conf), conf)
         elif self.confidence_type != "clip-max-prob":
             raise NotImplementedError(f"confidence_type={self.confidence_type}")
-        loss = F.cross_entropy(corr.transpose(2, 1), label, reduction="none")
         all_num = self._by_layer((conf > 1e-32).sum(dim=1)) + 1e-32
+        e = outputs["text_correlation_embedding"]
+        if self._shared_text(e):
+            # the (C, 512) superset matrix once for all scenes and layers: raw logits on the wgmma GEMM, normalisation,
+            # scale and the confidence-weighted CE in one row kernel (and one backward)
+            text = targets["text_features_clip"][0]
+            wloss = ops.text_contrastive_ce(e.reshape(-1, e.shape[-1]), text, label.reshape(-1), conf.reshape(-1),
+                                            targets["logit_scale"]).view(label.shape)
+            return {"loss_feat_seen_softmax_weakly_loss_with_novel_cate_confi":
+                    self._by_layer(wloss.sum(dim=1)) / all_num}
+        e = e / (e.norm(dim=-1, keepdim=True) + 1e-32)
+        text = targets["text_features_clip"].to(torch.float32)
+        corr = torch.bmm(e, text.permute(0, 2, 1)) * targets["logit_scale"]
+        loss = F.cross_entropy(corr.transpose(2, 1), label, reduction="none")
         return {"loss_feat_seen_softmax_weakly_loss_with_novel_cate_confi":
                 self._by_layer((loss * conf).sum(dim=1)) / all_num}
 
@@ -252,6 +267,8 @@ class SetCriterion(nn.Module):
             for k in self._PER_SCENE:
                 if isinstance(targets.get(k), torch.Tensor):
                     t = targets[k]
+                    if k == "text_features_clip" and self._shared_text(t):
+                        continue          # read as one shared matrix: nothing indexes it per scene
                     rep[k] = t.repeat(nlayers, *([1] * (t.dim() - 1)))
             targets = rep
         outputs["gious"] = generalized_box3d_iou(

@@ -148,6 +148,31 @@ def _class_prompts(args, evaluated=None):
     return [_prompt(c) for c in names[:n]]
 
 
+def superset_prompts(args):
+    """The 'superset' prompts of --if_clip_superset (reference :282-323): the seen classes' prompts, then the LVIS
+    names of ALL_SUPERCLASS_PATH (its first entry is the column header "name"), each prompt once.  The seen prompts are
+    the first 10 of the evaluated prompts for SUN RGB-D, and for ScanNet the seen classes' rows of the evaluated
+    prompts, in their order.  None when the class lists are not reachable (synthetic runs); FileNotFoundError when
+    they are and the LVIS list is not."""
+    evaluated = _class_prompts(args, True)
+    if evaluated is None:
+        return None
+    if not os.path.exists(ALL_SUPERCLASS_PATH):
+        raise FileNotFoundError(f"--if_clip_superset needs the LVIS class list {ALL_SUPERCLASS_PATH}, which is "
+                                "missing: refusing to stand random rows in for the superset text features")
+    if getattr(args, "dataset_name", "").find("scannet") != -1:
+        train = [int(i) for i in args.train_range_list]
+        ids = scannet_prompt_class_ids(train, [int(i) for i in args.test_range_list], int(args.reset_scannet_num))
+        seen = [evaluated[r] for r, c in enumerate(ids) if c in train]
+    else:
+        seen = evaluated[:10]
+    out = []
+    for p in seen + [_prompt(c) for c in list(np.load(ALL_SUPERCLASS_PATH, allow_pickle=True))[1:]]:
+        if p not in out:
+            out.append(p)
+    return out
+
+
 class Model3DETRPredictedBoxDistillationHead(nn.Module):
     """pre_encoder (PointNet++ SA) -> encoder -> query sampling -> decoder -> MLP heads,
     plus CLIP embeddings of the predicted boxes' image crops as distillation targets."""
@@ -244,6 +269,8 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
 
         evaluated = self._evaluated_prompts(args)
         prompts = _class_prompts(args, evaluated)
+        if self.if_clip_superset:
+            self.superset_all_classes_keys = superset_prompts(args)
         tokens = None
         if prompts is not None:
             try:
@@ -273,13 +300,25 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
             src = raw if self.TEXT_NORM_IN_CLIP_DTYPE else feats
             self.text_features_fg_norm = (src / src.norm(dim=1, keepdim=True)).to(torch.float32)
             if self.if_clip_superset:
-                nsup = getattr(args, "superset_size", 1201)
-                g = torch.Generator().manual_seed(4321)
-                sup = torch.randn(nsup, feats.shape[1], generator=g).to(self.device)
-                sup[: min(10, feats.shape[0])] = feats[: min(10, feats.shape[0])]
-                self.superset_text_features_fg_norm = sup / sup.norm(dim=1, keepdim=True)
+                if self.superset_all_classes_keys is not None and tokens is not None:
+                    self.superset_text_features_fg_norm = self.encode_prompts(self.superset_all_classes_keys)
+                else:       # synthetic run (no class lists): seeded random rows, warned about above
+                    nsup = getattr(args, "superset_size", 1201)
+                    g = torch.Generator().manual_seed(4321)
+                    sup = torch.randn(nsup, feats.shape[1], generator=g).to(self.device)
+                    sup[: min(10, feats.shape[0])] = feats[: min(10, feats.shape[0])]
+                    self.superset_text_features_fg_norm = sup / sup.norm(dim=1, keepdim=True)
             self.test_text_features_fg_norm = (self.superset_text_features_fg_norm if self.if_clip_superset
                                                else self.text_features_fg_norm)
+
+    @torch.no_grad()
+    def encode_prompts(self, prompts):
+        """(len(prompts), D) fp32 L2-normalised CLIP text features of `prompts` (reference :356-360): the text tower's
+        output cast to fp32, then normalised in fp32."""
+        from ..clip.tokenizer import tokenize
+
+        feats = self.clip_model.encode_text(tokenize(prompts).to(self.device)).to(torch.float32)
+        return feats / feats.norm(dim=1, keepdim=True)
 
     def to_device(self, device):
         """`.to(device)` plus the plain-tensor attributes the reference keeps outside buffers
@@ -691,9 +730,12 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
 
         if self.if_with_clip_train and (not if_real_test) and (not if_cmp_class) and (not if_test):
             bsz = point_clouds.shape[0]
-            text = (self.superset_text_features_fg_norm if self.if_clip_superset
-                    else self.text_features_fg_norm[: self.train_range_max, :])
-            out["text_features_clip"] = text.unsqueeze(0).repeat(bsz, 1, 1)
+            if self.if_clip_superset:
+                # every scene reads the same (C, D) superset matrix: a view, not B copies of it
+                out["text_features_clip"] = self.superset_text_features_fg_norm.unsqueeze(0).expand(bsz, -1, -1)
+            else:
+                out["text_features_clip"] = self.text_features_fg_norm[: self.train_range_max, :].unsqueeze(0).repeat(
+                    bsz, 1, 1)
             if self.online_nms_update_save_novel_label_clip_driven_with_cate_confidence:
                 out["maybe_novel_text_features_clip"] = (self.superset_text_features_fg_norm if self.if_clip_superset
                                                          else self.text_features_fg_norm[: self.test_range_max, :])

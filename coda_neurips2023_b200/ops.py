@@ -1296,6 +1296,80 @@ class Linear(torch.nn.Linear):
         return linear(x, self.weight, self.bias)
 
 
+# --------------------------------------------------------------------------- contrastive CE over a text matrix
+class _TextCE(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, s, e, label, w, scale, c):
+        rows, ld = s.shape
+        d = e.shape[1]
+        loss = torch.empty(rows, dtype=torch.float32, device=s.device)
+        lse, inv = torch.empty_like(loss), torch.empty_like(loss)
+        with torch.cuda.device(s.device):
+            check(lib().coda_text_ce_fwd(_ll(rows), _i(c), _i(ld), _i(d), ptr(s), ptr(e), ptr(label), ptr(w),
+                                         ptr(scale), ptr(loss), ptr(lse), ptr(inv), stream_of(s)), "text_ce_fwd")
+        ctx.save_for_backward(s, e, label, w, scale, lse, inv)
+        ctx.c = c
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        s, e, label, w, scale, lse, inv = ctx.saved_tensors
+        rows, ld = s.shape
+        d = e.shape[1]
+        gc = _f32c(g)
+        ds, dnorm = torch.empty_like(s), torch.empty_like(e)
+        with torch.cuda.device(s.device):
+            check(lib().coda_text_ce_bwd(_ll(rows), _i(ctx.c), _i(ld), _i(d), ptr(s), ptr(e), ptr(label), ptr(w),
+                                         ptr(scale), ptr(lse), ptr(inv), ptr(gc), ptr(ds), ptr(dnorm), stream_of(s)),
+                  "text_ce_bwd")
+        return ds, dnorm, None, None, None, None
+
+
+def text_ce_rows(s: torch.Tensor, e: torch.Tensor, label: torch.Tensor, w: torch.Tensor, scale: torch.Tensor,
+                 c: int) -> torch.Tensor:
+    """(rows,) w_r * CE(scale * S_r / (||e_r|| + 1e-32), label_r) from the raw logits S (rows, ld) = e T^T, columns
+    [0, c) used, and the embeddings e (rows, d) they came from (include/coda_step.h coda_text_ce_fwd).  Gradients flow
+    to S and, through the normalisation, to e; label -100 is ignored, other labels outside [0, c) give NaN."""
+    _need_cuda(s, "text_ce_rows")
+    assert s.dim() == 2 and e.dim() == 2 and s.shape[0] == e.shape[0] and s.shape[1] % 4 == 0 and 1 <= c <= s.shape[1]
+    assert label.numel() == s.shape[0] and w.numel() == s.shape[0] and scale.numel() == 1
+    assert not w.requires_grad and not scale.requires_grad
+    return _TextCE.apply(_f32c(s), _f32c(e), label.to(torch.int64).contiguous(), _f32c(w).reshape(-1),
+                         _f32c(scale.reshape(1)), c)
+
+
+_PADDED_TEXT: dict = {}
+
+
+def _rows_padded4(t: torch.Tensor) -> torch.Tensor:
+    """(C, D) -> (pad4(C), D) with zero rows appended, cached: the padded text matrix is a GEMM B operand whose
+    output rows TMA can store in place.  The entry keeps the source alive so that its address is not recycled."""
+    c = t.shape[0]
+    if c % 4 == 0:
+        return t
+    key = (t.data_ptr(), tuple(t.shape), t.stride(), t._version)
+    hit = _PADDED_TEXT.get(key)
+    if hit is None:
+        if len(_PADDED_TEXT) > 8:
+            _PADDED_TEXT.clear()
+        padded = torch.zeros(((c + 3) // 4 * 4, t.shape[1]), dtype=torch.float32, device=t.device)
+        padded[:c].copy_(t.detach())
+        hit = _PADDED_TEXT[key] = (padded, t)
+    return hit[0]
+
+
+def text_contrastive_ce(e: torch.Tensor, text: torch.Tensor, label: torch.Tensor, w: torch.Tensor,
+                        scale: torch.Tensor) -> torch.Tensor:
+    """(rows,) weighted cross-entropy of the stage-2 contrastive loss over ONE shared text matrix (criterion.py
+    loss_feat_seen_softmax_weakly_loss_with_novel_cate_confi): e (rows, D) the head's embeddings, text (C, D) the
+    normalised text features (no gradient).  The raw logits e T^T come from the wgmma GEMM (ops.linear, whose backward
+    gives dS T), the normalisation, scale, softmax and label pick from coda_text_ce_fwd / _bwd."""
+    _need_cuda(e, "text_contrastive_ce")
+    c = text.shape[0]
+    s = linear(e, _rows_padded4(text.to(torch.float32)))
+    return text_ce_rows(s, e, label, w, scale, c)
+
+
 # --------------------------------------------------------------------------- decoder memory K / V bank
 def pack_weights_concat(ws, nsplit: int) -> torch.Tensor:
     """Operand planes of the row-wise concatenation of the weights `ws` (each (n_i, k), row stride free):

@@ -76,6 +76,30 @@ int coda_masked_l1_bwd(int layers, long long rows, int d, const float *pred, con
                        const float *g, float *dpred, void *stream);
 
 /*
+ * Row-wise cross-entropy of the stage-2 contrastive loss over a shared text matrix (criterion.py
+ * loss_feat_seen_softmax_weakly_loss_with_novel_cate_confi, reference criterion.py:598-644), on raw logits
+ * S = e T^T that a GEMM has already written:
+ *   S     (rows, ld) fp32, columns [0, c) used, ld % 4 == 0, ld >= c;  e (rows, d) fp32 the un-normalised embeddings,
+ *   d % 4 == 0;  label (rows) int64;  w (rows) fp32 the per-row weights;  scale one device fp32 (logit scale, clipped).
+ * Forward, per row r:
+ *   inv[r] = 1 / (||e_r|| + 1e-32),  z_rc = scale * inv[r] * S_rc,  lse[r] = log sum_c exp(z_rc),
+ *   loss[r] = w[r] * (lse[r] - z_{r, label[r]});  label -100 -> loss 0 (ignore_index); any other label outside
+ *   [0, c) -> NaN.
+ * Backward, with g (rows) = dL / dloss and G_rc = g[r] * w[r] * (softmax_rc - [c == label[r]]):
+ *   dS_rc = scale * inv[r] * G_rc for c < c, 0 for c <= col < ld;
+ *   dnorm[r] = coef_r * e_r with coef_r = -(inv[r] / ||e_r||) * sum_c G_rc z_rc  (0 for a zero row): the
+ *   gradient through the normalisation, which the caller adds to the GEMM's dS T.  A label -100 row gets zeros,
+ *   an out-of-range label NaN.
+ * One warp per row, fixed lane-strided order and shuffle trees: the same bits on every run.  No atomics, no
+ * allocation, no synchronisation.
+ */
+int coda_text_ce_fwd(long long rows, int c, int ld, int d, const float *S, const float *e, const long long *label,
+                     const float *w, const float *scale, float *loss, float *lse, float *inv, void *stream);
+int coda_text_ce_bwd(long long rows, int c, int ld, int d, const float *S, const float *e, const long long *label,
+                     const float *w, const float *scale, const float *lse, const float *inv, const float *g,
+                     float *dS, float *dnorm, void *stream);
+
+/*
  * Global-norm gradient clip + AdamW over ONE flat fp32 parameter buffer.
  *
  * coda_grad_norm: state[1] = ||grad * grad_scale||_2 over the `n` elements (deterministic two-stage sum, fp64
