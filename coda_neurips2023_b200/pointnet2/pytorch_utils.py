@@ -120,10 +120,16 @@ class SharedMLP(nn.Sequential):
             for name, mod in block.named_children():
                 if isinstance(mod, nn.Conv2d):
                     if mod.kernel_size != (1, 1):
+                        if self.training and ops.bn_sync_world() > 1:
+                            raise NotImplementedError("synchronised BatchNorm after a convolution wider than 1x1")
                         return super().forward(x)
                     h = ops.linear(h, mod.weight.reshape(mod.weight.shape[0], -1), mod.bias)
                 elif isinstance(mod, _NormWrap):
-                    h = _batch_norm_rows(mod[0], h)
+                    if mod[0].training and ops.bn_sync_world() > 1:
+                        # synchronised statistics over every rank's rows (or NotImplementedError), never per-GPU ones
+                        h = ops.bn_act_rows(h, mod[0], relu=False, drop_p=0.0, training=True)
+                    else:
+                        h = _batch_norm_rows(mod[0], h)
                 elif isinstance(mod, nn.ReLU):
                     h = torch.relu(h)
                 else:

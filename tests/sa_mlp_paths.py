@@ -12,6 +12,7 @@ from __future__ import annotations
 THREADS = 256                 # threads per row-kernel block (sa_mlp_kernels.cu: THREADS)
 MAX_BLOCKS = 132 * 4          # grid_for's cap (sa_mlp_kernels.cu: MAX_BLOCKS)
 MAXPOOL_BLOCKS = 132 * 8      # coda_bn_relu_maxpool_rows's cap (sa_mlp_kernels.cu: its `grid`)
+COLSUM_BLOCKS = 132           # coda_rows_colsum's cap on grid_for (sa_mlp_kernels.cu: `if (grid > 132)`)
 
 # every width _channels_ok accepts: c % 4 == 0 and c / 4 divides 256
 WIDTHS = tuple(4 << i for i in range(9))      # 4, 8, ..., 1024
@@ -83,6 +84,16 @@ def maxpool_grid(groups: int) -> int:
 def strided(rows: int, c: int) -> bool:
     """a grid_for-launched kernel whose grid-stride loop takes a second iteration"""
     return rows > grid_for(rows, c) * slots(c)
+
+
+def colsum_grid(rows: int, c: int) -> int:
+    """sa_mlp_kernels.cu: the grid of colsum_partial_kernel in coda_rows_colsum"""
+    return min(grid_for(rows, c), COLSUM_BLOCKS)
+
+
+def colsum_strided(rows: int, c: int) -> bool:
+    """colsum_partial_kernel's grid-stride loop takes a second iteration"""
+    return rows > colsum_grid(rows, c) * slots(c)
 
 
 def node_launches(cin: int, widths, b: int, npoint: int, group: int):

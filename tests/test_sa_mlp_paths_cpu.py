@@ -85,3 +85,48 @@ def test_row_kernel_cases_reach_every_width_and_grid_stride():
     # the step's own shape: the max-pool grid strides over its 4095 groups
     assert any(k == "maxpool" and s and c == 256 for k, _, c, s in launches)
     assert set(E.OFFSET_RATIOS) >= {10, 30}
+
+
+def test_sync_bn_and_colsum_cases_reach_every_width_and_grid_stride():
+    """tests/test_sync_bn_gpu.py: coda_bn_rows_sums (bn_stats_partial_kernel on grid_for's grid) and coda_rows_colsum
+    (colsum_partial_kernel on at most 132 blocks) at every width, with and without a second grid-stride step; the
+    simulated ranks at every width; the GEMM partials of a plain first layer, of AFFINE_RELU layers, and of both the
+    B-resident and the tiled grid"""
+    import gemm_instances as G
+    import test_sync_bn_gpu as S
+
+    for cases, strided in ((S.SUMS_CASES, P.strided), (S.COLSUM_CASES, P.colsum_strided)):
+        assert {c for c, _ in cases} == set(P.WIDTHS)
+        for width in P.WIDTHS:
+            mine = [rows for c, rows in cases if c == width]
+            assert any(strided(rows, width) for rows in mine), width
+            assert any(not strided(rows, width) for rows in mine), width
+            assert 2 in mine, width
+            if P.slots(width) > 1:
+                assert any(rows % P.slots(width) for rows in mine), width
+    # colsum: exactly a full capped grid, and one row past it
+    for width in P.WIDTHS:
+        full = P.COLSUM_BLOCKS * P.slots(width)
+        assert {full, full + 1} <= {rows for c, rows in S.COLSUM_CASES if c == width}, width
+        assert P.colsum_grid(full, width) == P.COLSUM_BLOCKS and not P.colsum_strided(full, width)
+        assert P.colsum_strided(full + 1, width)
+    assert P.colsum_grid(1 << 20, 64) == 132 and P.grid_for(1 << 20, 64) == P.MAX_BLOCKS
+    # the step's pre-encoder row count at 64, 128 and 256 channels
+    assert {(c, 8 * 2048 * 64) for c in (64, 128, 256)} <= set(S.SUMS_CASES)
+    # simulated ranks: 2, 3 and 8 at every width, from row passes and from GEMM partials
+    assert {w for w, *_ in S.RANK_CASES} == {2, 3, 8}
+    for w in (2, 3, 8):
+        assert {c for ww, src, c, _ in S.RANK_CASES if ww == w and src == "rows"} == set(P.WIDTHS)
+        assert any(ww == w and src == "gemm" for ww, src, *_ in S.RANK_CASES)
+    # GEMM partials
+    resident = {G.gemm_a32(ns, m, n, k, False, mode, True)[1] for ns, m, n, k, mode in S.PARTIAL_CASES}
+    assert resident == {True, False}
+    assert {mode for *_, mode in S.PARTIAL_CASES} == {G.A32_PLAIN, G.A32_AFFINE_RELU}
+    assert any(G.gemm_a32(ns, m, n, k, False, mode, True)[1] and mode == G.A32_AFFINE_RELU
+               for ns, m, n, k, mode in S.PARTIAL_CASES)
+    # the node on gloo ranks: statistics from a row pass (small-K first layer) and from GEMM partials
+    assert {P.small_k(spec[0]) is None for spec, *_ in S.NODE_RANK_CASES} == {True, False}
+    for spec, b, npoint, group, x_grad in S.NODE_RANK_CASES:
+        assert P.applicable(spec[0], spec[1:], group, x_grad)
+    # the masked encoder's interim MLP (259 -> 256 -> 256 -> 256) is declined by the fused node
+    assert not P.applicable(S.ENC_DIM + 3, [256, 256, S.ENC_DIM], S.ENC_NSAMPLE, False)
