@@ -23,11 +23,12 @@ novel_candidates_kernel(int q, int g, int cap, const int *__restrict__ boxes2d, 
                         const float *__restrict__ objectness, const float *__restrict__ pred_corners,
                         const float *__restrict__ gt_corners, const float *__restrict__ gt_present, float nms_iou,
                         float gt_iou, float min_objectness, int *__restrict__ cand_idx, int *__restrict__ cand_count) {
-  extern __shared__ unsigned char smem_raw[];
+  extern __shared__ __align__(16) unsigned char smem_raw[];
   const int words = (q + 31) / 32;
-  float *score = reinterpret_cast<float *>(smem_raw);            // [q]
-  float4 *box = reinterpret_cast<float4 *>(score + q);           // [q]  (x1, y1, x2, y2), in score order
-  int *order = reinterpret_cast<int *>(box + q);                 // [q]  rank -> box index
+  // the float4 array first: it stays 16-byte aligned for every q, not only for q % 4 == 0
+  float4 *box = reinterpret_cast<float4 *>(smem_raw);            // [q]  (x1, y1, x2, y2), in score order
+  float *score = reinterpret_cast<float *>(box + q);             // [q]
+  int *order = reinterpret_cast<int *>(score + q);               // [q]  rank -> box index
   uint32_t *sup = reinterpret_cast<uint32_t *>(order + q);       // [q][words]  suppression bits (row a: later boxes b)
   uint32_t *keep = sup + (size_t)q * words;                      // [words]
   unsigned char *ok = reinterpret_cast<unsigned char *>(keep + words);   // [q] survives gt filter + thresholds
@@ -36,13 +37,16 @@ novel_candidates_kernel(int q, int g, int cap, const int *__restrict__ boxes2d, 
   // scores: objectness, -1 for a box that was given up (degenerate crop / behind the camera / zero size)
   for (int i = tid; i < q; i += blockDim.x) score[i] = valid[(size_t)b * q + i] ? objectness[(size_t)b * q + i] : -1.0f;
   __syncthreads();
-  // descending order (ties: lower index first), by counting
+  // rank by counting, in a total order so that the ranks are a permutation for any input: NaN above every number, then
+  // descending value, ties (NaN with NaN, -0.0 with +0.0) by lower index -- torchvision.ops.nms's stable sort
   for (int i = tid; i < q; i += blockDim.x) {
     const float s = score[i];
+    const bool sn = isnan(s);
     int r = 0;
     for (int j = 0; j < q; ++j) {
       const float t = score[j];
-      r += (t > s) || (t == s && j < i);
+      const bool tn = isnan(t);
+      r += tn != sn ? tn : (t > s) || (!(t < s) && j < i);
     }
     order[r] = i;
   }

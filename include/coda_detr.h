@@ -135,10 +135,13 @@ int coda_hungarian(int b, int nprop, int ngt, const float *cost, const int *nact
  *   boxes2d (b, q, 4) int32 projected boxes, valid (b, q) uint8 (0 = box given up: its NMS box is the dummy
  *   (0, 0, 2, 2) and its score -1, as in the reference), objectness (b, q), pred_corners (b, q, 8, 3),
  *   gt_corners (b, g, 8, 3), gt_present (b, g) in {0, 1}.
- *   A box is a candidate iff it survives the class-agnostic 2-D NMS (IoU > nms_iou suppresses, score order, ties by
- *   index), is valid, has objectness >= min_objectness and its axis-aligned 3-D IoU with every present ground-truth
- *   box is <= gt_iou.  cand_idx (b, cap) int32: candidate box indices in descending score order, -1 padded;
+ *   A box is a candidate iff it survives the class-agnostic 2-D NMS (IoU > nms_iou suppresses, score order), is
+ *   valid, has objectness >= min_objectness (a NaN objectness is not below it) and its axis-aligned 3-D IoU with every
+ *   present ground-truth box is <= gt_iou.  The score order is total, like the stable descending sort of
+ *   torchvision.ops.nms: NaN above every number, then descending value, ties (NaN with NaN, -0.0 with +0.0) by lower
+ *   index.  cand_idx (b, cap) int32: candidate box indices in that order, -1 padded;
  *   cand_count (b, 2) int32: entries written, and the untruncated total (total > written: raise `cap`).
+ *   q from 1 to 1024 and cap >= 1 (CODA_EINVAL otherwise).
  */
 int coda_novel_candidates(int b, int q, int g, int cap, const int *boxes2d, const unsigned char *valid,
                           const float *objectness, const float *pred_corners, const float *gt_corners,
