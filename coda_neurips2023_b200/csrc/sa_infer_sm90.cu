@@ -44,6 +44,15 @@ constexpr int SMEM_W3 = W3_PLANES * (C2 / 64) * W3_TILE;   // 128 KB
 constexpr int AFFINE_FLOATS = 2 * (C1 + C2 + C3);          // scale1 shift1 scale2 shift2 scale3 shift3
 constexpr int POOL_FLOATS = 2 * 2 * 4 * 128;               // [warpgroup][half][warp][128 columns]
 
+// max(a, b) that returns NaN when either is NaN (fmaxf drops a NaN operand).  Every ReLU and the max over neighbours
+// use it: the module path (relu, F.max_pool2d) carries a NaN through, so a non-finite neighbour makes NaN, not
+// plausible features.  One FMNMX either way.
+__device__ __forceinline__ float max_nan(float a, float b) {
+  float d;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+  return d;
+}
+
 // layer-3 plane products (A plane, B plane), smallest terms first
 __host__ __device__ constexpr int l3_a(int p) { return p == 0 ? 1 : p == 1 ? 2 : p == 2 ? 1 : 0; }
 __host__ __device__ constexpr int l3_b(int p) { return p == 0 ? 1 : p == 1 ? 0 : p == 2 ? 0 : p == 3 ? 1 : 0; }
@@ -141,8 +150,8 @@ sa_infer_kernel(const __grid_constant__ InferMaps maps, const InferParams P) {
           v0 = fmaf(w.x, xin[c][i], v0);
           v1 = fmaf(w.y, xin[c][i], v1);
         }
-        v0 = fmaxf(fmaf(v0, s1[col], h1[col]), 0.f);
-        v1 = fmaxf(fmaf(v1, s1[col + 1], h1[col + 1]), 0.f);
+        v0 = max_nan(fmaf(v0, s1[col], h1[col]), 0.f);
+        v1 = max_nan(fmaf(v1, s1[col + 1], h1[col + 1]), 0.f);
         uint32_t w[3];
         split_pair<3>(v0, v1, w);
 #pragma unroll
@@ -175,8 +184,8 @@ sa_infer_kernel(const __grid_constant__ InferMaps maps, const InferParams P) {
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         const int i = q & 1, c = 2 * kk + (q >> 1), col = c * 8 + 2 * t4;
-        const float v0 = fmaxf(fmaf(acc2[c * 4 + i * 2], s2[col], h2[col]), 0.f);
-        const float v1 = fmaxf(fmaf(acc2[c * 4 + i * 2 + 1], s2[col + 1], h2[col + 1]), 0.f);
+        const float v0 = max_nan(fmaf(acc2[c * 4 + i * 2], s2[col], h2[col]), 0.f);
+        const float v1 = max_nan(fmaf(acc2[c * 4 + i * 2 + 1], s2[col + 1], h2[col + 1]), 0.f);
         uint32_t w[3];
         split_pair<3>(v0, v1, w);
 #pragma unroll
@@ -208,12 +217,12 @@ sa_infer_kernel(const __grid_constant__ InferMaps maps, const InferParams P) {
       for (int c = 0; c < 16; ++c) {
         const int col = h * 128 + c * 8 + 2 * t4;
         const float sc0 = s3[col], sh0 = h3[col], sc1 = s3[col + 1], sh1 = h3[col + 1];
-        float m0 = fmaxf(fmaf(acc3[c * 4], sc0, sh0), fmaf(acc3[c * 4 + 2], sc0, sh0));
-        float m1 = fmaxf(fmaf(acc3[c * 4 + 1], sc1, sh1), fmaf(acc3[c * 4 + 3], sc1, sh1));
+        float m0 = max_nan(fmaf(acc3[c * 4], sc0, sh0), fmaf(acc3[c * 4 + 2], sc0, sh0));
+        float m1 = max_nan(fmaf(acc3[c * 4 + 1], sc1, sh1), fmaf(acc3[c * 4 + 3], sc1, sh1));
 #pragma unroll
         for (int o = 4; o < 32; o <<= 1) {       // the warp's 16 rows: lane bits 2..4
-          m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, o));
-          m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, o));
+          m0 = max_nan(m0, __shfl_xor_sync(0xffffffffu, m0, o));
+          m1 = max_nan(m1, __shfl_xor_sync(0xffffffffu, m1, o));
         }
         if (g == 0) *reinterpret_cast<float2 *>(buf + warp * 128 + c * 8 + 2 * t4) = make_float2(m0, m1);
       }
@@ -221,8 +230,8 @@ sa_infer_kernel(const __grid_constant__ InferMaps maps, const InferParams P) {
       // later, after the barrier of the other half, which every thread reaches only after reading it.
       bar_sync(1 + wg, 128);
       const int tl = tid & 127;
-      const float m = fmaxf(fmaxf(buf[tl], buf[128 + tl]), fmaxf(buf[256 + tl], buf[384 + tl]));
-      orow[h * 128 + tl] = fmaxf(m, 0.f);
+      const float m = max_nan(max_nan(buf[tl], buf[128 + tl]), max_nan(buf[256 + tl], buf[384 + tl]));
+      orow[h * 128 + tl] = max_nan(m, 0.f);
     }
   }
 }

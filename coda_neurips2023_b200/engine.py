@@ -730,6 +730,9 @@ class TrainStep:
                 elif k == "pseudo_box_path":
                     self.static_batch[k] = v
             self.graph.replay()
+            # the replayed AdamW wrote the parameters through the flat buffer: neither their version counters nor the
+            # weight-plane epoch moved, so planes an eager forward (evaluation) packed since the last step are stale
+            ops.invalidate_weight_cache()
             out = self.static_out
         else:
             out = self._body(batch, curr_epoch)

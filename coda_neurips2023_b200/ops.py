@@ -1078,7 +1078,9 @@ _ACT_CACHE: dict = {}   # packed planes of activations that several layers consu
 
 def invalidate_weight_cache() -> None:
     """Call after parameters were updated through storage the tensors' version counters do not see
-    (the flat-buffer optimiser step of engine.TrainStep).  Also ends the per-step activation-pack cache."""
+    (the flat-buffer optimiser step of engine.TrainStep, eager or replayed from its CUDA graph: a replay runs no
+    Python, so TrainStep.__call__ calls this after every replay).  Also ends the per-step activation-pack cache.
+    Host-only: no synchronisation, no launch."""
     global _WEIGHT_EPOCH
     _WEIGHT_EPOCH += 1
     _WEIGHT_CACHE.clear()

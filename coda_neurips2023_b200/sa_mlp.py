@@ -307,6 +307,7 @@ def shared_mlp_max(x_rows: torch.Tensor, blocks, group: int, nsplit: int | None 
 # The one layout the inference kernel covers (csrc/sa_infer_sm90.cu): the 3DETR pre-encoder, xyz (+ rgb) input.
 INFER_WIDTHS = (64, 128, 256)
 INFER_GROUP = 64
+INFER_PLANES = 3          # bf16 planes packed per weight (coda_sa_mlp_max_infer's w2_planes / w3_planes)
 
 
 def infer_applicable(x: torch.Tensor, blocks, group: int) -> bool:
@@ -350,8 +351,9 @@ def shared_mlp_max_infer(x: torch.Tensor, blocks, group: int) -> torch.Tensor:
     b, c0, npoint, nsample = x.shape
     (conv1, _), (conv2, _), (conv3, _) = blocks
     w1 = conv1.weight.detach().reshape(INFER_WIDTHS[0], c0).contiguous()
-    w2 = ops._packed_weight(conv2.weight.reshape(INFER_WIDTHS[1], -1), False, ops.DEFAULT_NSPLIT)
-    w3 = ops._packed_weight(conv3.weight.reshape(INFER_WIDTHS[2], -1), False, ops.DEFAULT_NSPLIT)
+    # the kernel reads 3 planes of W2 and planes 0 and 1 of W3, whatever ops.DEFAULT_NSPLIT says
+    w2 = ops._packed_weight(conv2.weight.reshape(INFER_WIDTHS[1], -1), False, INFER_PLANES)
+    w3 = ops._packed_weight(conv3.weight.reshape(INFER_WIDTHS[2], -1), False, INFER_PLANES)
     affine = _folded_affine(blocks)
     out = torch.empty((b * npoint, INFER_WIDTHS[2]), dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):
