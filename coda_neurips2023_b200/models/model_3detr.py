@@ -42,6 +42,8 @@ CLIP_CHECKPOINT = "./CLIP/pretrain_models/ViT-B-16.pt"  # path the reference har
 ALL_CLASS_PATH_V1 = "datasets/all_classes_trainval_v1.npy"
 ALL_CLASS_PATH_V2 = "datasets/all_classes_trainval_v2_revised_del_val_less_than_5_classes.npy"
 ALL_SUPERCLASS_PATH = "datasets/lvis_1204.npy"
+ALL_CMP_CLASS_PATH = "datasets/ov_3detr.npy"                  # the OV-3DET paper's comparison classes, SUN RGB-D
+ALL_CMP_CLASS_PATH_SCANNET = "datasets/ov_3detr_scannet.npy"  # ... and ScanNet
 SCANNET_CLASS_NAMES_PATH = "datasets/scannet_200_classname_no_wall_floor.npy"   # the text rows, in order
 SCANNET_CLASS_IDS_PATH = "datasets/scannet_200_class2id.npy"                     # {name: ScanNet-200 class id}
 
@@ -173,6 +175,19 @@ def superset_prompts(args):
     return out
 
 
+def cmp_prompts(args):
+    """The prompts of the comparison classes of forward(if_cmp_class=True) (reference :1971-2000): the names of
+    ALL_CMP_CLASS_PATH (ALL_CMP_CLASS_PATH_SCANNET when dataset_name contains "scannet") in file order.  None when the
+    class lists are not reachable (synthetic runs); FileNotFoundError when they are and the comparison list is not."""
+    if _class_prompts(args, True) is None:
+        return None
+    path = ALL_CMP_CLASS_PATH_SCANNET if getattr(args, "dataset_name", "").find("scannet") != -1 else ALL_CMP_CLASS_PATH
+    if not os.path.exists(path):
+        raise FileNotFoundError(f"the comparison-class evaluation (if_cmp_class) needs the class list {path}, "
+                                "which is missing")
+    return [_prompt(c) for c in np.load(path)]
+
+
 class Model3DETRPredictedBoxDistillationHead(nn.Module):
     """pre_encoder (PointNet++ SA) -> encoder -> query sampling -> decoder -> MLP heads,
     plus CLIP embeddings of the predicted boxes' image crops as distillation targets."""
@@ -282,6 +297,7 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
                                        f"missing ({e}): refusing to substitute random text features") from e
                 tokens = None
         self.all_classes_keys = prompts
+        self.text_features_synthetic = tokens is None
         with torch.no_grad():
             if tokens is not None:
                 raw = self.clip_model.encode_text(tokens)
@@ -326,7 +342,8 @@ class Model3DETRPredictedBoxDistillationHead(nn.Module):
         self.to(device)
         self.device = str(device)
         for name in ("text_features_fg", "text_features_fg_norm", "superset_text_features_fg_norm",
-                     "test_text_features_fg_norm", "test_logit_scale", "logit_scale"):
+                     "test_text_features_fg_norm", "cmp_text_features_fg", "cmp_text_features_fg_norm",
+                     "test_logit_scale", "logit_scale"):
             if isinstance(getattr(self, name, None), torch.Tensor) and name not in self._parameters:
                 setattr(self, name, getattr(self, name).to(device))
         if str(device) == "cpu" and self.has_clip:
@@ -823,6 +840,38 @@ class Model3DETRMultiClassHead(Model3DETRPredictedBoxDistillationHead):
     def _evaluated_prompts(self, args):
         return True                          # reference :1923-1988: always the test_range_max / evaluated classes
 
+    # seed of the random comparison-class rows of synthetic runs
+    CMP_SYNTHETIC_SEED = 2468
+
+    def _build_clip(self, args, dataset_config):
+        super()._build_clip(args, dataset_config)
+        self.build_cmp_text(args)
+
+    @torch.no_grad()
+    def build_cmp_text(self, args):
+        """The text matrix of forward(if_cmp_class=True), encoded once (reference :2092-2095) and normalised as
+        text_features_fg_norm is (in CLIP's dtype, then fp32): `cmp_text_features_fg` and `cmp_text_features_fg_norm`
+        (C, D), plain tensors, so that checkpoints gain no state-dict key.  Where the class text is synthetic (warned
+        about by _build_clip), C seeded random rows stand in: 20 for SUN RGB-D, 19 for ScanNet.  A missing comparison
+        list does not stop the build, which serves every other evaluation: the first if_cmp_class forward raises."""
+        self.all_cmp_classes_keys = self.cmp_text_features_fg = self.cmp_text_features_fg_norm = None
+        self._cmp_text_error = None
+        if self.text_features_synthetic:
+            n = 19 if getattr(args, "dataset_name", "").find("scannet") != -1 else 20
+            g = torch.Generator().manual_seed(self.CMP_SYNTHETIC_SEED)
+            raw = torch.randn(n, self.clip_model.visual.output_dim, generator=g).to(self.device)
+        else:
+            try:
+                self.all_cmp_classes_keys = cmp_prompts(args)
+            except FileNotFoundError as e:
+                self._cmp_text_error = str(e)
+                return
+            from ..clip.tokenizer import tokenize
+
+            raw = self.clip_model.encode_text(tokenize(self.all_cmp_classes_keys).to(self.device))
+        self.cmp_text_features_fg = raw.to(torch.float32)
+        self.cmp_text_features_fg_norm = (raw / raw.norm(dim=1, keepdim=True)).to(torch.float32)
+
     def build_mlp_heads(self, dataset_config, decoder_dim, mlp_dropout):
         # reference :2145-2176: objectness (1 + 1 logits) and the box geometry
         mlp_func = partial(GenericMLP, norm_fn_name="bn1d", activation="relu", use_conv=True,
@@ -836,17 +885,19 @@ class Model3DETRMultiClassHead(Model3DETRPredictedBoxDistillationHead):
         ])
 
     def _clip_outputs(self, inputs, box_predictions, if_test, if_real_test, if_cmp_class, curr_epoch):
-        # reference :3903-3926
-        if if_cmp_class:
-            raise NotImplementedError("the baseline head does not implement if_cmp_class")
+        # reference :3903-3930
         out = box_predictions["outputs"]
         out["logit_scale"] = torch.clip(self.logit_scale.exp(), min=None, max=100)
-        if not (if_real_test or if_test):
+        if not (if_real_test or if_cmp_class or if_test):
             text = (self.superset_text_features_fg_norm if self.if_clip_superset
                     else self.text_features_fg_norm[: self.train_range_max, :])
             out["text_features_clip"] = text.unsqueeze(0).repeat(inputs["point_clouds"].shape[0], 1, 1)
         if if_real_test:
             self.classify_boxes(inputs, out)
+        if if_cmp_class:
+            if self.cmp_text_features_fg_norm is None:
+                raise FileNotFoundError(self._cmp_text_error)
+            self.classify_boxes(inputs, out, text=self.cmp_text_features_fg_norm)
         return box_predictions
 
     def _camera_inputs(self, inputs, bsz: int, dev):
@@ -886,9 +937,10 @@ class Model3DETRMultiClassHead(Model3DETRPredictedBoxDistillationHead):
                                   self._camera_inputs(inputs, bsz, corners.device), extent=extent, **camera)
 
     @torch.no_grad()
-    def classify_boxes(self, inputs, out):
-        """out['sem_cls_prob'] (B, Q, test_range_max) = softmax(logit_scale * f_hat . text^T) of the CLIP feature f of
-        each box's crop, zeros for a box without a usable crop; out['sem_cls_logits'] zeros (reference :2810-3085).
+    def classify_boxes(self, inputs, out, text=None):
+        """out['sem_cls_prob'] (B, Q, C) = softmax(logit_scale * f_hat . text^T) of the CLIP feature f of each box's
+        crop, zeros for a box without a usable crop; out['sem_cls_logits'] zeros (reference :2810-3085).  `text` is
+        the (C, D) normalised text matrix: by default the evaluated classes' (C = test_range_max).
         The usable boxes are compacted on the device (one read of their count per batch) and only their crops go
         through the tower, CROPS_PER_CALL at a time."""
         bsz, nq = out["box_corners_xyz"].shape[:2]
@@ -898,7 +950,8 @@ class Model3DETRMultiClassHead(Model3DETRPredictedBoxDistillationHead):
         n = idx.numel()
         row_map = torch.full((bsz * nq,), -1, dtype=torch.int32, device=dev)
         row_map[idx] = torch.arange(n, dtype=torch.int32, device=dev)
-        text = self.text_features_fg_norm
+        if text is None:
+            text = self.text_features_fg_norm
         feats = torch.empty((n, text.shape[1]), dtype=torch.float32, device=dev)
         flat_boxes = boxes.reshape(-1, 4)
         for s in range(0, n, self.CROPS_PER_CALL):

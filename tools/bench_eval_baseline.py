@@ -3,11 +3,13 @@
 730 x 531 images, a random-init ViT-B/16 (the tower's real 197-token geometry), 46 classes; then the ScanNet shape
 (1296 x 968 images, 60 classes) once.
 
-    python tools/bench_eval_baseline.py [--reps N]
+    python tools/bench_eval_baseline.py [--reps N] [--cmp]
 
 Prints JSON lines: the card (name, power limit, max SM clock); per shape the eval forward with and without the
 classification step (CUDA events, median), the usable crops per batch, the crop + tower + classify time alone, the
-tower's algorithmic TFLOP/s (FLOPs from the shapes below) and the peak allocated memory."""
+tower's algorithmic TFLOP/s (FLOPs from the shapes below) and the peak allocated memory.  With --cmp, per shape instead
+the eval forward of the comparison-class evaluation (if_cmp_class: 20 / 19 classes) and of the real-test one on the same
+model and batch, alternated (CUDA events, median of N each)."""
 import argparse
 import json
 import subprocess
@@ -61,7 +63,8 @@ def timed(fn, reps):
     return median(ts)
 
 
-def bench(shape, reps):
+def setup(shape):
+    """The model (weights filled by name) and batch of a shape."""
     if shape == "sunrgbd":
         over, hw, camera = dict(dataset_name="sunrgbd_image", test_range_max=46), (531, 730), "sunrgbd"
     else:
@@ -78,6 +81,11 @@ def bench(shape, reps):
     model.to_device("cuda")
     model.eval()
     batch = synthetic.to_device(synthetic.make_batch(SCENES, POINTS, seed=0, image_hw=hw, camera=camera), "cuda")
+    return args, model, batch, hw
+
+
+def bench(shape, reps):
+    args, model, batch, hw = setup(shape)
     with torch.no_grad():
         def with_cls():
             return model(batch, if_real_test=True)
@@ -105,11 +113,43 @@ def bench(shape, reps):
             "peak_allocated_gib": round(peak / 2 ** 30, 2)}
 
 
+def bench_cmp(shape, reps):
+    """The comparison-class pass (forward(if_cmp_class=True): 20 SUN RGB-D / 19 ScanNet classes) next to the real-test
+    pass (46 / 60 classes) on the same model and batch, alternated.  Both crop and encode the same boxes; only the
+    text matrix of the classify kernel differs."""
+    _, model, batch, hw = setup(shape)
+    with torch.no_grad():
+        def real_test():
+            return model(batch, if_real_test=True)
+
+        def cmp_class():
+            return model(batch, if_cmp_class=True)
+
+        real, cmp = real_test()["outputs"], cmp_class()["outputs"]
+        t_real, t_cmp = [], []
+        for i in range(reps):           # alternated, each pass first in every other round
+            if i % 2:
+                t_cmp.append(timed(cmp_class, 1))
+            t_real.append(timed(real_test, 1))
+            if not i % 2:
+                t_cmp.append(timed(cmp_class, 1))
+    return {"shape": shape, "scenes": SCENES, "points": POINTS, "queries": QUERIES, "image_hw": list(hw),
+            "usable_crops": int(cmp["clip_usable_mask"].sum()), "real_test_classes": real["sem_cls_prob"].shape[-1],
+            "cmp_classes": cmp["sem_cls_prob"].shape[-1], "real_test_eval_forward_ms": round(median(t_real), 2),
+            "cmp_eval_forward_ms": round(median(t_cmp), 2), "reps": reps}
+
+
 def main():
     p = argparse.ArgumentParser()
     p.add_argument("--reps", type=int, default=5)
+    p.add_argument("--cmp", action="store_true",
+                   help="time the comparison-class pass (if_cmp_class) next to the real-test pass instead")
     a = p.parse_args()
     print(json.dumps(card()), flush=True)
+    if a.cmp:
+        print(json.dumps(bench_cmp("sunrgbd", a.reps)), flush=True)
+        print(json.dumps(bench_cmp("scannet", a.reps)), flush=True)
+        return
     print(json.dumps(bench("sunrgbd", a.reps)), flush=True)
     print(json.dumps(bench("scannet", 2)), flush=True)
 
