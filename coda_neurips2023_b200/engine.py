@@ -20,8 +20,10 @@ object, laid out for the H100:
     save_checkpoint / resume_if_possible carry the optimizer state through unchanged;
   * rank 0's parameters and buffers are broadcast before the first step (what DDP's constructor does;
     the reference seeds every rank differently, main.py:982-985);
-  * BatchNorm statistics stay per GPU (no SyncBatchNorm): the step's only other collective is the
-    4-byte box-count all-reduce of the criterion;
+  * BatchNorm statistics stay per GPU by default: the step's only other collective is the 4-byte box-count
+    all-reduce of the criterion.  `sync_bn=True` synchronises plain BatchNorm modules; the nn.SyncBatchNorm
+    modules of a model that went through convert_sync_batchnorm always synchronise over their own process group
+    (ops.bn_sync_group);
   * the batch is copied from pinned host memory on the compute stream and the loss is left on the
     device: the caller decides when to synchronise.
 """
@@ -438,10 +440,12 @@ class TrainStep:
 
     def __init__(self, args, model, criterion, device, nbuckets: int = 4, sync_bn: bool | None = None,
                  optimizer: torch.optim.AdamW | None = None):
-        """sync_bn: synchronise BatchNorm statistics over the ranks (the reference converts to SyncBatchNorm when
-        ngpus > 1, main.py:993).  Default (None -> args.sync_bn, else False): per-GPU statistics and exactly one
-        gradient all-reduce per step, as the north-star asks; True adds one small all-reduce per BatchNorm layer
-        and direction (DESIGN.md section 7) and makes N ranks x B scenes equal one rank x N*B scenes.
+        """sync_bn: synchronise the statistics of plain BatchNorm modules over the ranks (the reference converts to
+        SyncBatchNorm when ngpus > 1, main.py:993).  Default (None -> args.sync_bn, else False): per-GPU statistics
+        and exactly one gradient all-reduce per step; True adds one small all-reduce per BatchNorm layer and
+        direction (DESIGN.md section 7) and makes N ranks x B scenes equal one rank x N*B scenes.  The
+        nn.SyncBatchNorm modules of a converted model (the reference's `model_no_ddp` after convert_sync_batchnorm)
+        synchronise over their own process group whatever this says, as torch's SyncBatchNorm does.
 
         optimizer: the caller's torch.optim.AdamW over the model's trainable parameters (the reference's
         build_optimizer), possibly holding a loaded state.  `prepare` adopts it: its moments and step count become

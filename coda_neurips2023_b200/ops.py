@@ -494,18 +494,24 @@ def bn_channels_ok(c: int) -> bool:
     return 4 <= c <= 1024 and c % 4 == 0 and 256 % (c // 4) == 0
 
 
-# ---- synchronised BatchNorm (reference main.py:993 convert_sync_batchnorm): an OPTION of this package -- the default
-# is per-GPU statistics and exactly one gradient all-reduce per step (DESIGN.md section 7).  When on, every BatchNorm
-# executed by bn_act_rows / sa_mlp takes its batch statistics over all ranks: one 16*C-byte fp64 all-reduce per layer
-# forward, one 8*C-byte fp32 all-reduce backward.  Equal row counts per rank (fixed batch per GPU) are assumed.
+# ---- synchronised BatchNorm (reference main.py:993 convert_sync_batchnorm).  Which group, if any, a BatchNorm
+# synchronises over is decided per module by bn_sync_group(): an nn.SyncBatchNorm follows the rules of torch's
+# SyncBatchNorm.forward (its own process_group); a plain BatchNorm follows this package's global option, off by default
+# (per-GPU statistics and exactly one gradient all-reduce per step, DESIGN.md section 7).  A synchronised BatchNorm
+# executed by bn_act_rows / sa_mlp takes its batch statistics over the group's ranks: one 16*C-byte fp64 all-reduce
+# per layer forward, one 8*C-byte fp32 all-reduce backward.  Every rank of the group is assumed to hold the same
+# number of rows (the finalize divides by rows * world): the reference's DistributedSampler pads the dataset so that
+# every rank gets the same batch size.  No collective checks it.
 _BN_SYNC = {"on": False, "group": None}
 
 
 def set_bn_sync(enabled: bool, group=None) -> None:
+    """The global option for plain (unconverted) BatchNorm modules; nn.SyncBatchNorm modules ignore it."""
     _BN_SYNC["on"], _BN_SYNC["group"] = bool(enabled), group
 
 
 def bn_sync_world() -> int:
+    """Ranks the global option synchronises plain BatchNorm modules over (1: off, or no process group)."""
     import torch.distributed as dist
 
     if not _BN_SYNC["on"] or not dist.is_available() or not dist.is_initialized():
@@ -513,15 +519,39 @@ def bn_sync_world() -> int:
     return dist.get_world_size(_BN_SYNC["group"])
 
 
-def bn_stats_synced(rows: int, c: int, bn, momentum: float, track: bool, gamma, beta, want_affine: bool, *, y=None,
-                    partials=None):
-    """Global batch statistics: local fp64 column sums (from y, or from a GEMM epilogue's partials) -> all-reduce ->
-    finalize over rows * world.  Returns (mean, invstd, scale | None, shift | None)."""
+def bn_sync_group(bn):
+    """The process group whose ranks' rows `bn` takes its batch statistics over, or None for statistics of this rank's
+    rows alone.  An nn.SyncBatchNorm synchronises, as torch's SyncBatchNorm.forward does, in training mode with a process
+    group initialised and more than one rank in `bn.process_group` (None: the default group); otherwise it takes the
+    statistics of this rank's rows.  A plain BatchNorm synchronises whenever it takes batch statistics (training mode,
+    or eval mode without running statistics) while the global option is on (set_bn_sync / TrainStep(sync_bn=True))
+    over more than one rank."""
+    import torch.distributed as dist
+
+    if not dist.is_available() or not dist.is_initialized():
+        return None
+    if isinstance(bn, torch.nn.SyncBatchNorm):
+        if not bn.training:
+            return None
+        group = bn.process_group
+    elif _BN_SYNC["on"] and (bn.training or bn.running_mean is None):
+        group = _BN_SYNC["group"]
+    else:
+        return None
+    group = dist.group.WORLD if group is None else group
+    return group if dist.get_world_size(group) > 1 else None
+
+
+def bn_stats_synced(group, rows: int, c: int, bn, momentum: float, track: bool, gamma, beta, want_affine: bool, *,
+                    y=None, partials=None):
+    """Batch statistics over the ranks of `group` (bn_sync_group): local fp64 column sums (from y, or from a GEMM
+    epilogue's partials) -> all-reduce -> finalize over rows * world.  Returns (mean, invstd, scale | None,
+    shift | None)."""
     import torch.distributed as dist
 
     src = y if y is not None else partials
     dev = src.device
-    world = bn_sync_world()
+    world = dist.get_world_size(group)
     sums = torch.empty(2 * c, dtype=torch.float64, device=dev)
     mean = torch.empty(c, dtype=torch.float32, device=dev)
     invstd = torch.empty(c, dtype=torch.float32, device=dev)
@@ -537,7 +567,7 @@ def bn_stats_synced(rows: int, c: int, bn, momentum: float, track: bool, gamma, 
         else:
             check(L.coda_bn_partials_sums(_i(partials.shape[0]), _i(c), ptr(partials), ptr(sums), stream_of(partials)),
                   "bn_partials_sums")
-        dist.all_reduce(sums, group=_BN_SYNC["group"])
+        dist.all_reduce(sums, group=group)
         check(L.coda_bn_stats_finalize_sums(_ll(rows * world), _i(c), ptr(sums), _f(bn.eps), _f(momentum),
                                             ptr(bn.running_mean if track else None),
                                             ptr(bn.running_var if track else None), ptr(gamma), ptr(beta), ptr(mean),
@@ -545,14 +575,14 @@ def bn_stats_synced(rows: int, c: int, bn, momentum: float, track: bool, gamma, 
     return mean, invstd, scale, shift
 
 
-def bn_sync_backward_sums(s1: torch.Tensor, s2: torch.Tensor):
+def bn_sync_backward_sums(s1: torch.Tensor, s2: torch.Tensor, group):
     """(s1, s2) = local sums of dz and dz * xhat (they ARE dbeta / dgamma and stay local, as in torch's SyncBatchNorm);
-    the input gradient needs the global means: returns the rank-averaged copies (the kernels divide by the local row
-    count, so average = global sum / global count)."""
+    the input gradient needs the means over the ranks of `group`: returns the rank-averaged copies (the kernels divide
+    by the local row count, so average = global sum / global count)."""
     import torch.distributed as dist
 
     t = torch.stack((s1, s2))
-    dist.all_reduce(t, op=dist.ReduceOp.AVG, group=_BN_SYNC["group"])
+    dist.all_reduce(t, op=dist.ReduceOp.AVG, group=group)
     return t[0], t[1]
 
 
@@ -572,10 +602,11 @@ class _BNActRows(torch.autograd.Function):
             raise NotImplementedError("cumulative-average BatchNorm momentum is not on the CoDA path")
         out = torch.empty_like(yc)
         L = lib()
-        ctx.sync = bn_sync_world() > 1
+        ctx.group = bn_sync_group(bn)
         with torch.cuda.device(dev):
-            if ctx.sync:
-                mean, invstd, _, _ = bn_stats_synced(rows, c, bn, float(bn.momentum), track, gamma, beta, False, y=yc)
+            if ctx.group is not None:
+                mean, invstd, _, _ = bn_stats_synced(ctx.group, rows, c, bn, float(bn.momentum), track, gamma, beta,
+                                                     False, y=yc)
             else:
                 mean = torch.empty(c, dtype=torch.float32, device=dev)
                 invstd = torch.empty(c, dtype=torch.float32, device=dev)
@@ -610,7 +641,7 @@ class _BNActRows(torch.autograd.Function):
         with torch.cuda.device(dev):
             check(L.coda_bn_act_rows_bwd_reduce(*args, ptr(s1), ptr(s2), ptr(_bn_scratch(c, dev)), stream_of(y)),
                   "bn_act_rows_bwd_reduce")
-            t1, t2 = bn_sync_backward_sums(s1, s2) if ctx.sync else (s1, s2)
+            t1, t2 = bn_sync_backward_sums(s1, s2, ctx.group) if ctx.group is not None else (s1, s2)
             check(L.coda_bn_act_rows_bwd(*args, ptr(t1), ptr(t2), ptr(dy), stream_of(y)), "bn_act_rows_bwd")
         if sg is not None:
             return dy, _sunk(sg), _sunk(sb), None, None, None, None
@@ -621,12 +652,9 @@ def bn_act_rows(h: torch.Tensor, bn: torch.nn.modules.batchnorm._BatchNorm, relu
                 training: bool) -> torch.Tensor:
     """drop(relu(bn(h))) for h (rows, C): the BatchNorm1d -> ReLU -> Dropout run of a GenericMLP block
     (reference models/helpers.py:82-99) as two kernels.  Training-mode statistics come from the batch (and update
-    the running buffers); eval mode normalises with the running statistics."""
+    the running buffers, over the ranks of bn_sync_group(bn) when it names a group); eval mode normalises with the
+    running statistics.  `bn` may be an nn.BatchNorm1d or the nn.SyncBatchNorm convert_sync_batchnorm made of one."""
     _need_cuda(h, "bn_act_rows")
-    if isinstance(bn, torch.nn.SyncBatchNorm):
-        raise NotImplementedError("torch SyncBatchNorm modules are not executed by this package: keep the BatchNorm "
-                                  "modules and switch synchronisation on with ops.set_bn_sync(True) / "
-                                  "TrainStep(sync_bn=True) (DESIGN.md section 7)")
     c = h.shape[-1]
     if not (bn.affine and bn_channels_ok(c)):
         raise NotImplementedError(f"BatchNorm over {c} channels without affine parameters is not on the CoDA path")

@@ -104,6 +104,14 @@ def _batch_norm_rows(bn: nn.modules.batchnorm._BatchNorm, h: torch.Tensor) -> to
                         bn.weight, bn.bias, use_batch, momentum, bn.eps)
 
 
+def _is_bn2d(slot) -> bool:
+    """Does a block's `_NormWrap` slot hold a 2-D BatchNorm: an nn.BatchNorm2d, or the nn.SyncBatchNorm that
+    convert_sync_batchnorm put in its place?  A SyncBatchNorm has no dimensionality of its own: the slot (this
+    module's BatchNorm2d wrapper) gives it."""
+    return isinstance(slot, _NormWrap) and (isinstance(slot[0], nn.BatchNorm2d)
+                                            or (isinstance(slot, BatchNorm2d) and isinstance(slot[0], nn.SyncBatchNorm)))
+
+
 class SharedMLP(nn.Sequential):
     """Stack of 1x1 Conv2d blocks: `layer0`, `layer1`, ... (reference
     pytorch_utils.py:8-33).  Executed channels-last: the (B, C, npoint, nsample) map is
@@ -120,12 +128,13 @@ class SharedMLP(nn.Sequential):
             for name, mod in block.named_children():
                 if isinstance(mod, nn.Conv2d):
                     if mod.kernel_size != (1, 1):
-                        if self.training and ops.bn_sync_world() > 1:
+                        norms = [m[0] for m in self.modules() if isinstance(m, _NormWrap)]
+                        if any(ops.bn_sync_group(bn) is not None for bn in norms):
                             raise NotImplementedError("synchronised BatchNorm after a convolution wider than 1x1")
                         return super().forward(x)
                     h = ops.linear(h, mod.weight.reshape(mod.weight.shape[0], -1), mod.bias)
                 elif isinstance(mod, _NormWrap):
-                    if mod[0].training and ops.bn_sync_world() > 1:
+                    if ops.bn_sync_group(mod[0]) is not None:
                         # synchronised statistics over every rank's rows (or NotImplementedError), never per-GPU ones
                         h = ops.bn_act_rows(h, mod[0], relu=False, drop_p=0.0, training=True)
                     else:
@@ -140,20 +149,17 @@ class SharedMLP(nn.Sequential):
         """relu(bn(conv(.))) blocks followed by the max over the last (nsample) axis, as one fused autograd
         node (sa_mlp.shared_mlp_max): (B, C, npoint, nsample) -> (B, C_out, npoint).  Returns None when the
         fused path does not apply (CPU, eval mode, other block layouts); the caller then runs forward() and
-        pools itself."""
+        pools itself.  The BatchNorm of a block may be the nn.SyncBatchNorm convert_sync_batchnorm made of it
+        (the `_NormWrap` slot says it is 2-D); the node synchronises it as ops.bn_sync_group says."""
         from .. import sa_mlp
 
-        if any(isinstance(m, nn.SyncBatchNorm) for m in self.modules()):
-            raise NotImplementedError("SyncBatchNorm inside SharedMLP: this package runs per-GPU BatchNorm "
-                                      "(DESIGN.md section 7) -- do not call convert_sync_batchnorm on the model")
         if x.dim() != 4 or not x.is_cuda or not torch.is_grad_enabled():
             return None
         blocks = []
         for block in self:
             mods = list(block.children())
             if (len(mods) != 3 or not isinstance(mods[0], nn.Conv2d) or mods[0].kernel_size != (1, 1)
-                    or not isinstance(mods[1], _NormWrap) or not isinstance(mods[1][0], nn.BatchNorm2d)
-                    or not isinstance(mods[2], nn.ReLU)):
+                    or not _is_bn2d(mods[1]) or not isinstance(mods[2], nn.ReLU)):
                 return None
             blocks.append((mods[0], mods[1][0]))
         b, c, p, s = x.shape
@@ -177,8 +183,7 @@ class SharedMLP(nn.Sequential):
         for block in self:
             mods = list(block.children())
             if (len(mods) != 3 or not isinstance(mods[0], nn.Conv2d) or mods[0].kernel_size != (1, 1)
-                    or not isinstance(mods[1], _NormWrap) or not isinstance(mods[1][0], nn.BatchNorm2d)
-                    or not isinstance(mods[2], nn.ReLU)):
+                    or not _is_bn2d(mods[1]) or not isinstance(mods[2], nn.ReLU)):
                 return None
             blocks.append((mods[0], mods[1][0]))
         b, _, p, s = x.shape

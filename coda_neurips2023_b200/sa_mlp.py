@@ -88,8 +88,9 @@ def _stats_affine(y: torch.Tensor, bn, gamma, beta):
     rows, c = y.shape
     momentum, track = _bn_bookkeeping(bn)
     dev = y.device
-    if ops.bn_sync_world() > 1:
-        return ops.bn_stats_synced(rows, c, bn, momentum, track, gamma, beta, True, y=y)
+    group = ops.bn_sync_group(bn)
+    if group is not None:
+        return ops.bn_stats_synced(group, rows, c, bn, momentum, track, gamma, beta, True, y=y)
     cpad = ops._pad64(c)
     mean = torch.empty(c, dtype=torch.float32, device=dev)
     invstd = torch.empty(c, dtype=torch.float32, device=dev)
@@ -119,8 +120,9 @@ def _stats_from_partials(partials: torch.Tensor, rows: int, bn, gamma, beta, wan
     nblocks, _, c = partials.shape
     momentum, track = _bn_bookkeeping(bn)
     dev = partials.device
-    if ops.bn_sync_world() > 1:
-        return ops.bn_stats_synced(rows, c, bn, momentum, track, gamma, beta, want_affine, partials=partials)
+    group = ops.bn_sync_group(bn)
+    if group is not None:
+        return ops.bn_stats_synced(group, rows, c, bn, momentum, track, gamma, beta, want_affine, partials=partials)
     mean = torch.empty(c, dtype=torch.float32, device=dev)
     invstd = torch.empty(c, dtype=torch.float32, device=dev)
     scale = shift = None
@@ -179,7 +181,7 @@ class _SharedMLPMax(torch.autograd.Function):
                                                       ptr(gamma), ptr(beta), ptr(pooled), ptr(argmax), stream_of(x)),
                           "bn_relu_maxpool_rows")
         ctx.nl, ctx.group, ctx.small_k, ctx.nsplit = nl, group, small_k, nsplit
-        ctx.sync = ops.bn_sync_world() > 1
+        ctx.groups = [ops.bn_sync_group(bn) for bn in bns]
         ctx.save_for_backward(x, argmax, *ys, *means, *invstds, *scales, *shifts, *params)
         ctx.mark_non_differentiable(argmax)
         return pooled, argmax
@@ -228,11 +230,11 @@ class _SharedMLPMax(torch.autograd.Function):
                                                     ptr(gamma), ptr(beta), ptr(s1), ptr(s2), ptr(scratch), stream_of(x)),
                           "bn_relu_bwd_reduce")
                 loc1, loc2 = s1, s2
-                if ctx.sync:
+                if ctx.groups[li] is not None:
                     # the input gradient needs the means over every rank's rows; dgamma / dbeta stay the local sums.
                     # Taken BEFORE the sink is notified: the notification may start the all-reduce of that range of
                     # the flat gradient on the side stream, which rewrites s1 / s2 in place
-                    s1, s2 = ops.bn_sync_backward_sums(s1, s2)
+                    s1, s2 = ops.bn_sync_backward_sums(s1, s2, ctx.groups[li])
                 if sg is None:
                     grads[3 * li + 1], grads[3 * li + 2] = loc2, loc1    # dgamma, dbeta
                 else:
@@ -294,7 +296,8 @@ class _SharedMLPMax(torch.autograd.Function):
 
 def shared_mlp_max(x_rows: torch.Tensor, blocks, group: int, nsplit: int | None = None) -> torch.Tensor:
     """x_rows (R, C0) channels-last grouped features -> (R / group, C_last): max over each run of `group` rows of
-    relu(bn(conv(...))).  `blocks` = [(conv, bn), ...] (1x1 Conv2d without bias, BatchNorm2d in training mode)."""
+    relu(bn(conv(...))).  `blocks` = [(conv, bn), ...] (1x1 Conv2d without bias, BatchNorm2d or SyncBatchNorm in
+    training mode)."""
     params = []
     for conv, bn in blocks:
         params += [conv.weight.reshape(conv.weight.shape[0], -1), bn.weight, bn.bias]
