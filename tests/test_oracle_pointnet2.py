@@ -20,15 +20,20 @@ def _bitrev(v: np.ndarray, bits: int) -> np.ndarray:
     return out
 
 
-def fps_position_space(xyz: np.ndarray, m: int) -> np.ndarray:
-    """Independent formulation used by the CUDA kernel: argmax of temp with ties
-    broken by the smallest position p = bitrev(k mod bs) * R + k div bs."""
-    b, n, _ = xyz.shape
+def fps_positions(n: int) -> np.ndarray:
+    """Position p = bitrev(k mod bs) * R + k div bs of every point k of an n-point scene."""
     bs = orc.opt_n_threads(n)
     bits = int(np.log2(bs))
     R = (n + bs - 1) // bs
     k = np.arange(n)
-    pos = _bitrev(k % bs, bits) * R + k // bs
+    return _bitrev(k % bs, bits) * R + k // bs
+
+
+def fps_position_space(xyz: np.ndarray, m: int) -> np.ndarray:
+    """Independent formulation used by the CUDA kernel: argmax of temp with ties
+    broken by the smallest position p = bitrev(k mod bs) * R + k div bs."""
+    b, n, _ = xyz.shape
+    pos = fps_positions(n)
     out = np.zeros((b, m), dtype=np.int32)
     for bi in range(b):
         p = xyz[bi].astype(np.float32)
