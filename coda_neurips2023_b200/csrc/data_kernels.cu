@@ -1,6 +1,7 @@
 // Data layer on the device (sm_90a): the per-scene numpy pipeline of the reference's dataset __getitem__
-// (datasets/sunrgbd_anonymous_aligned_image.py:618-795, utils/random_cuboid.py, utils/pc_util.py:24-32) for a whole
-// batch of raw scenes that are already resident in HBM:
+// (datasets/sunrgbd_anonymous_aligned_image.py:618-795, utils/random_cuboid.py, utils/pc_util.py:24-32) and of the
+// ScanNet item (datasets/scannet_anonymous_aligned_image.py:373-702) for a whole batch of raw scenes that are already
+// resident in HBM:
 //
 //   scene_transform   flip about the YZ plane, rotation about the up axis, isotropic scale of the points
 //                     (:660-705; the boxes -- a handful per scene -- follow on the host side of the module)
@@ -12,6 +13,8 @@
 //                     num_points draws WITHOUT a sort: a keyed Feistel permutation of [0, M) with cycle walking
 //                     (M >= num_points: without replacement; M < num_points: hashed draws with replacement), gather,
 //                     and the extent of the sampled cloud (point_cloud_dims_min / max)
+//   sample_points_ex  the same, plus the ScanNet item's extra gathers (positions in the cropped cloud, raw rows there)
+//   flip2_rotate_scale  ScanNet: flips about YZ and XZ, rotation with a float64 matrix, float64 scale (:545-604)
 //   image_augment     flip, per-channel brightness and colour shift, per-pixel jitter, clip, back to uint8 (:624-655)
 //
 // Randomness is the caller's: candidate tables, angles, seeds arrive as small device arrays (drawn with numpy on the
@@ -238,17 +241,21 @@ __device__ __forceinline__ uint32_t feistel(uint32_t x, int half_bits, uint32_t 
 // out[b][i] = points[list[perm_b(i)]]  (all `stride` columns), i < nsample.  M >= nsample: perm = Feistel bijection
 // on the next power of four >= M, cycle-walked back into [0, M) -- distinct indices, no sort.  M < nsample: hashed
 // draws (with replacement, like np.random.choice(..., replace=True)).  choice (b, nsample) = index into the raw scene.
+// kEx (the ScanNet item, datasets/scannet_anonymous_aligned_image.py:507-532) also writes list_pos = perm_b(i), the
+// position in the cropped cloud, and rgb_out[b][i] = the first rgb_stride columns of the RAW scene's row list_pos --
+// the reference indexes the uncropped scene with the cropped cloud's choices.
+template <bool kEx>
 __global__ void __launch_bounds__(256)
 sample_kernel(int nmax, int stride, int nsample, const float *__restrict__ pts, const int *__restrict__ list,
               const int *__restrict__ count, const uint32_t *__restrict__ seed, float *__restrict__ out,
-              int *__restrict__ choice) {
+              int *__restrict__ choice, int rgb_stride, int *__restrict__ list_pos, float *__restrict__ rgb_out) {
   const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nsample) return;
   const int m = count[b];
   int src = 0;
+  uint32_t j = 0;
   if (m > 0) {
     const uint32_t key = mix32d(seed[b] ^ 0xA511E9B3u);
-    uint32_t j;
     if (m >= nsample) {
       int half_bits = 1;
       while ((1u << (2 * half_bits)) < (uint32_t)m) ++half_bits;
@@ -263,6 +270,35 @@ sample_kernel(int nmax, int stride, int nsample, const float *__restrict__ pts, 
   float *o = out + ((size_t)b * nsample + i) * stride;
   for (int c = 0; c < stride; ++c) o[c] = m > 0 ? p[c] : 0.f;
   choice[(size_t)b * nsample + i] = m > 0 ? src : -1;
+  if (kEx) {
+    const float *q = pts + ((size_t)b * nmax + j) * stride;
+    float *r = rgb_out + ((size_t)b * nsample + i) * rgb_stride;
+    for (int c = 0; c < rgb_stride; ++c) r[c] = m > 0 ? q[c] : 0.f;
+    list_pos[(size_t)b * nsample + i] = m > 0 ? (int)j : -1;
+  }
+}
+
+// ------------------------------------------------------------------ ScanNet flips / rotation / scale
+// datasets/scannet_anonymous_aligned_image.py:545-604 on float32 rows: x <- -x (YZ flip), y <- -y (XZ flip), exact;
+// then np.dot(pc[:, 0:3], rot^T) with a float64 rot -- numpy promotes to float64 and BLAS accumulates the three
+// products with fused multiply-adds, the result is stored back as float32 -- and finally `pc[:, 0:3] *= scale`
+// with a float64 scale: float64 product, stored as float32.
+__global__ void __launch_bounds__(256)
+flip2_rotate_scale_kernel(int nmax, int stride, const int *__restrict__ npts, const float *__restrict__ flip_yz,
+                          const float *__restrict__ flip_xz, const double *__restrict__ rot,
+                          const double *__restrict__ scale, float *__restrict__ pts) {
+  const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nmax || (npts && i >= npts[b])) return;
+  float *p = pts + ((size_t)b * nmax + i) * stride;
+  const double *R = rot + b * 9;
+  const double x = (double)__fmul_rn(p[0], flip_yz[b]), y = (double)__fmul_rn(p[1], flip_xz[b]), z = (double)p[2];
+  const double s = scale[b];
+  float v[3];
+#pragma unroll
+  for (int j = 0; j < 3; ++j)
+    v[j] = __double2float_rn(__fma_rn(z, R[j * 3 + 2], __fma_rn(y, R[j * 3 + 1], __dmul_rn(x, R[j * 3]))));
+#pragma unroll
+  for (int j = 0; j < 3; ++j) p[j] = __double2float_rn(__dmul_rn((double)v[j], s));
 }
 
 // per-scene extent of the first three columns: dims (b, 6) = min xyz | max xyz
@@ -369,9 +405,38 @@ int coda_sample_points(int b, int nmax, int stride, int nsample, const int *npts
     return CODA_EINVAL;
   cudaStream_t s = (cudaStream_t)stream;
   compact_kernel<<<b, 1024, 0, s>>>(nmax, stride, npts, points, crop, list_scratch, count);
-  sample_kernel<<<dim3((nsample + 255) / 256, b), 256, 0, s>>>(nmax, stride, nsample, points, list_scratch, count, seed,
-                                                               out, choice);
+  sample_kernel<false><<<dim3((nsample + 255) / 256, b), 256, 0, s>>>(nmax, stride, nsample, points, list_scratch,
+                                                                      count, seed, out, choice, 0, nullptr, nullptr);
   extent_kernel<<<b, 256, 0, s>>>(nsample, stride, nullptr, out, dims);
+  return launch_status();
+}
+
+int coda_sample_points_ex(int b, int nmax, int stride, int nsample, int rgb_stride, const int *npts,
+                          const float *points, const double *crop, const unsigned int *seed, int *list_scratch,
+                          int *count, float *out, int *choice, int *list_pos, float *rgb_out, float *dims,
+                          void *stream) {
+  if (b < 0 || nmax <= 0 || stride < 3 || nsample <= 0 || rgb_stride < 0 || rgb_stride > stride) return CODA_EINVAL;
+  if (b == 0) return CODA_OK;
+  if (!npts || !points || !crop || !seed || !list_scratch || !count || !out || !choice || !list_pos || !dims ||
+      (rgb_stride > 0 && !rgb_out) || b > 65535)
+    return CODA_EINVAL;
+  cudaStream_t s = (cudaStream_t)stream;
+  compact_kernel<<<b, 1024, 0, s>>>(nmax, stride, npts, points, crop, list_scratch, count);
+  sample_kernel<true><<<dim3((nsample + 255) / 256, b), 256, 0, s>>>(nmax, stride, nsample, points, list_scratch,
+                                                                     count, seed, out, choice, rgb_stride, list_pos,
+                                                                     rgb_out);
+  extent_kernel<<<b, 256, 0, s>>>(nsample, stride, nullptr, out, dims);
+  return launch_status();
+}
+
+int coda_points_flip2_rotate_scale(int b, int nmax, int stride, const int *npts, const float *flip_yz,
+                                   const float *flip_xz, const double *rot, const double *scale, float *points,
+                                   void *stream) {
+  if (b < 0 || nmax < 0 || stride < 3) return CODA_EINVAL;
+  if (b == 0 || nmax == 0) return CODA_OK;
+  if (!flip_yz || !flip_xz || !rot || !scale || !points || b > 65535) return CODA_EINVAL;
+  flip2_rotate_scale_kernel<<<dim3((nmax + 255) / 256, b), 256, 0, (cudaStream_t)stream>>>(
+      nmax, stride, npts, flip_yz, flip_xz, rot, scale, points);
   return launch_status();
 }
 

@@ -1,2 +1,3 @@
 """Device-side data layer (SURVEY.md section 8 row f4): see device_pipeline.py."""
-from .device_pipeline import DeviceSceneAugmentor, draw_augmentation  # noqa: F401
+from .device_pipeline import (DeviceScanNetAugmentor, DeviceSceneAugmentor, draw_augmentation,  # noqa: F401
+                              draw_augmentation_scannet)

@@ -1,7 +1,9 @@
 /*
  * coda_data.h -- C-ABI of the device-side data layer (SURVEY.md section 8 row f4): the per-scene numpy pipeline of
- * the reference's dataset __getitem__ (datasets/sunrgbd_anonymous_aligned_image.py:618-795 and its ScanNet twin,
- * utils/random_cuboid.py, utils/pc_util.py:24-32) for a batch of raw scenes resident in HBM.  Conventions as in
+ * the reference's SUN RGB-D dataset __getitem__ (datasets/sunrgbd_anonymous_aligned_image.py:618-795,
+ * utils/random_cuboid.py, utils/pc_util.py:24-32) and of its ScanNet item (datasets/scannet_anonymous_aligned_image.py
+ * :373-702, which crops and samples the raw scene first and transforms the sampled rows last, see
+ * coda_sample_points_ex and coda_points_flip2_rotate_scale) for a batch of raw scenes resident in HBM.  Conventions as in
  * coda_pointnet2.h.  Scenes are padded: points (b, nmax, stride) fp32 with npts (b) valid rows (columns 0-2 = xyz,
  * the others -- colour, height -- travel along); boxes (b, gmax, box_stride) fp32 rows [cx, cy, cz, ...] with
  * nbox (b) valid rows.  All randomness comes in as small device arrays drawn by the caller.
@@ -49,6 +51,31 @@ int coda_random_cuboid(int b, int nmax, int stride, int ncand, int gmax, int box
 int coda_sample_points(int b, int nmax, int stride, int nsample, const int *npts, const float *points,
                        const double *crop, const unsigned int *seed, int *list_scratch, int *count, float *out,
                        int *choice, float *dims, void *stream);
+
+/*
+ * coda_sample_points plus the ScanNet item's gathers (datasets/scannet_anonymous_aligned_image.py:507-532), in the same
+ *   pass and with the same draws, so out / choice / count / dims are those coda_sample_points gives:
+ *   list_pos (b, nsample) = position of each sample in the cropped cloud (the reference's `choices`; choice is the
+ *   raw-scene row, out[i] = points[choice[i]]); rgb_out (b, nsample, rgb_stride) = the first rgb_stride <= stride
+ *   columns of the RAW scene's row list_pos[i] -- the reference's point_clouds_rgb / pcl_color index the uncropped
+ *   scene with the cropped cloud's choices, and this reproduces it.  rgb_out may be NULL when rgb_stride is 0.
+ */
+int coda_sample_points_ex(int b, int nmax, int stride, int nsample, int rgb_stride, const int *npts,
+                          const float *points, const double *crop, const unsigned int *seed, int *list_scratch,
+                          int *count, float *out, int *choice, int *list_pos, float *rgb_out, float *dims,
+                          void *stream);
+
+/*
+ * In place on (b, nmax, stride) fp32 rows, npts (b) valid (NULL: all nmax): the ScanNet item's augmentation of the
+ *   sampled points (:545-604): x <- flip_yz * x, y <- flip_xz * y (flip_* (b) = +-1, exact), then xyz <- xyz @ rot^T
+ *   with rot (b, 3, 3) fp64, then xyz <- xyz * scale with scale (b) fp64; columns 3 and up are untouched.  Rounding
+ *   as numpy does it on a float32 cloud: the product with the float64 matrix is formed in fp64 as
+ *   fma(z, r2, fma(y, r1, x * r0)) (BLAS dgemm's order) and stored as float32; the scale product is formed in fp64
+ *   and stored as float32.  The extents come after this, from coda_points_extent.
+ */
+int coda_points_flip2_rotate_scale(int b, int nmax, int stride, const int *npts, const float *flip_yz,
+                                   const float *flip_xz, const double *rot, const double *scale, float *points,
+                                   void *stream);
 
 /*
  * Image augmentation of :624-655 on uint8 HWC images: horizontal flip (flip (b) != 0), per-channel gain (b, 3) and
