@@ -37,6 +37,16 @@ __device__ __forceinline__ uint32_t mix32d(uint32_t h) {
   return h;
 }
 
+// coordinate-type helpers: the float32 instantiations keep the exact operations they were written with (fminf /
+// fmaxf, __double2float_rn), the float64 ones (SUN RGB-D's float64 scene files) the same operations on doubles
+__device__ __forceinline__ float vmin(float a, float b) { return fminf(a, b); }
+__device__ __forceinline__ float vmax(float a, float b) { return fmaxf(a, b); }
+__device__ __forceinline__ double vmin(double a, double b) { return fmin(a, b); }
+__device__ __forceinline__ double vmax(double a, double b) { return fmax(a, b); }
+template <typename T> __device__ __forceinline__ T from_double(double v);
+template <> __device__ __forceinline__ float from_double<float>(double v) { return __double2float_rn(v); }
+template <> __device__ __forceinline__ double from_double<double>(double v) { return v; }
+
 // ------------------------------------------------------------------ flip / rotate / scale
 // xyz' = ((flip_x * x, y, z) @ rot^T) * scale, evaluated as numpy does on float32 arrays: products and sums rounded
 // separately, left to right (datasets/...:663-700: point_cloud[:, 0] *= -1; np.dot(pc, rot^T); pc *= scale)
@@ -60,14 +70,13 @@ scene_transform_kernel(int nmax, int stride, const int *__restrict__ npts, const
 // ------------------------------------------------------------------ RandomCuboid
 // stats[b][c] = {count, min x, min y, min z, max x, max y, max z} of the points inside candidate c
 // (random_cuboid.py:47-66: centre = a point of the cloud, half extent = range_xyz * crop_range / 2, inclusive bounds)
-struct CuboidStat { float v[8]; };
-
+template <typename T>
 __global__ void __launch_bounds__(256)
-cuboid_stats_kernel(int nmax, int stride, int ncand, const int *__restrict__ npts, const float *__restrict__ pts,
-                    const float *__restrict__ range_xyz, const double *__restrict__ crop_range,
-                    const float *__restrict__ center_u, float *__restrict__ stats) {
+cuboid_stats_kernel(int nmax, int stride, int ncand, const int *__restrict__ npts, const T *__restrict__ pts,
+                    const T *__restrict__ range_xyz, const double *__restrict__ crop_range,
+                    const float *__restrict__ center_u, T *__restrict__ stats) {
   const int b = blockIdx.y, c = blockIdx.x, n = min(npts[b], nmax);
-  const float *P = pts + (size_t)b * nmax * stride;
+  const T *P = pts + (size_t)b * nmax * stride;
   const double *cr = crop_range + ((size_t)b * ncand + c) * 3;
   int ci = (int)(center_u[(size_t)b * ncand + c] * (float)n);
   ci = ci < 0 ? 0 : (ci >= n ? n - 1 : ci);
@@ -81,25 +90,25 @@ cuboid_stats_kernel(int nmax, int stride, int ncand, const int *__restrict__ npt
     hi[a] = ctr + half;
   }
   int cnt = 0;
-  float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
+  T mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    const float x = P[(size_t)i * stride], y = P[(size_t)i * stride + 1], z = P[(size_t)i * stride + 2];
+    const T x = P[(size_t)i * stride], y = P[(size_t)i * stride + 1], z = P[(size_t)i * stride + 2];
     if ((double)x <= hi[0] && (double)y <= hi[1] && (double)z <= hi[2] && (double)x >= lo[0] && (double)y >= lo[1] &&
         (double)z >= lo[2]) {
       ++cnt;
-      mn[0] = fminf(mn[0], x); mn[1] = fminf(mn[1], y); mn[2] = fminf(mn[2], z);
-      mx[0] = fmaxf(mx[0], x); mx[1] = fmaxf(mx[1], y); mx[2] = fmaxf(mx[2], z);
+      mn[0] = vmin(mn[0], x); mn[1] = vmin(mn[1], y); mn[2] = vmin(mn[2], z);
+      mx[0] = vmax(mx[0], x); mx[1] = vmax(mx[1], y); mx[2] = vmax(mx[2], z);
     }
   }
   __shared__ int s_cnt[8];
-  __shared__ float s_mn[8][3], s_mx[8][3];
+  __shared__ T s_mn[8][3], s_mx[8][3];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
-      mn[a] = fminf(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
-      mx[a] = fmaxf(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
+      mn[a] = vmin(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
+      mx[a] = vmax(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
     }
   }
   const int w = threadIdx.x >> 5;
@@ -111,34 +120,35 @@ cuboid_stats_kernel(int nmax, int stride, int ncand, const int *__restrict__ npt
   if (threadIdx.x == 0) {
     for (int q = 1; q < (int)(blockDim.x >> 5); ++q) {
       cnt += s_cnt[q];
-      for (int a = 0; a < 3; ++a) { mn[a] = fminf(mn[a], s_mn[q][a]); mx[a] = fmaxf(mx[a], s_mx[q][a]); }
+      for (int a = 0; a < 3; ++a) { mn[a] = vmin(mn[a], s_mn[q][a]); mx[a] = vmax(mx[a], s_mx[q][a]); }
     }
-    float *o = stats + ((size_t)b * ncand + c) * 8;
-    o[0] = (float)cnt;
+    T *o = stats + ((size_t)b * ncand + c) * 8;
+    o[0] = (T)cnt;
     for (int a = 0; a < 3; ++a) { o[1 + a] = mn[a]; o[4 + a] = mx[a]; }
-    o[7] = 0.f;
+    o[7] = 0;
   }
 }
 
 // chosen[b] = index of the first candidate that passes every test of random_cuboid.py:42-86, or -1 (fallback:
 // the scene is kept whole); box_keep (b, gmax) = boxes whose centre lies within the extent of the kept points;
 // crop (b, 6) = the chosen cuboid's inclusive bounds (lo xyz, hi xyz)
+template <typename T>
 __global__ void __launch_bounds__(32)
 cuboid_pick_kernel(int nmax, int stride, int ncand, int gmax, int min_points, float aspect_min,
-                   const int *__restrict__ npts, const float *__restrict__ pts, const float *__restrict__ range_xyz,
+                   const int *__restrict__ npts, const T *__restrict__ pts, const T *__restrict__ range_xyz,
                    const double *__restrict__ crop_range, const float *__restrict__ center_u,
-                   const float *__restrict__ stats, const float *__restrict__ boxes, int box_stride,
+                   const T *__restrict__ stats, const T *__restrict__ boxes, int box_stride,
                    const int *__restrict__ nbox, int *__restrict__ chosen, double *__restrict__ crop,
                    unsigned char *__restrict__ box_keep) {
   const int b = blockIdx.x, lane = threadIdx.x;
   const int n = min(npts[b], nmax), ng = min(nbox[b], gmax);
-  const float *B = boxes + (size_t)b * gmax * box_stride;
-  // "target_boxes.sum() > 0": ground truth present at all (random_cuboid.py:74)
-  float bsum = 0.f;
+  const T *B = boxes + (size_t)b * gmax * box_stride;
+  // "target_boxes.sum() > 0": ground truth present at all (random_cuboid.py:74), summed in the boxes' type
+  T bsum = 0;
   for (int i = lane; i < ng * box_stride; i += 32) bsum += B[i];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) bsum += __shfl_xor_sync(0xffffffffu, bsum, o);
-  const bool has_boxes = bsum > 0.f;
+  const bool has_boxes = bsum > (T)0;
   int pick = -1;
   for (int c0 = 0; c0 < ncand && pick < 0; c0 += 32) {
     const int c = c0 + lane;
@@ -148,12 +158,12 @@ cuboid_pick_kernel(int nmax, int stride, int ncand, int gmax, int min_points, fl
       const double xy = fmin(cr[0], cr[1]) / fmax(cr[0], cr[1]);
       const double xz = fmin(cr[0], cr[2]) / fmax(cr[0], cr[2]);
       const double yz = fmin(cr[1], cr[2]) / fmax(cr[1], cr[2]);
-      const float *st = stats + ((size_t)b * ncand + c) * 8;
+      const T *st = stats + ((size_t)b * ncand + c) * 8;
       ok = (xy >= (double)aspect_min || xz >= (double)aspect_min || yz >= (double)aspect_min) && (int)st[0] >= min_points;
       if (ok && has_boxes) {
         bool any = false;
         for (int q = 0; q < ng; ++q) {
-          const float *bx = B + (size_t)q * box_stride;
+          const T *bx = B + (size_t)q * box_stride;
           any = any || (bx[0] >= st[1] && bx[1] >= st[2] && bx[2] >= st[3] && bx[0] <= st[4] && bx[1] <= st[5] && bx[2] <= st[6]);
         }
         ok = any;
@@ -164,9 +174,9 @@ cuboid_pick_kernel(int nmax, int stride, int ncand, int gmax, int min_points, fl
   }
   if (lane == 0) chosen[b] = pick;
   double lo[3] = {-INFINITY, -INFINITY, -INFINITY}, hi[3] = {INFINITY, INFINITY, INFINITY};
-  const float *st = pick >= 0 ? stats + ((size_t)b * ncand + pick) * 8 : nullptr;
+  const T *st = pick >= 0 ? stats + ((size_t)b * ncand + pick) * 8 : nullptr;
   if (pick >= 0) {
-    const float *P = pts + (size_t)b * nmax * stride;
+    const T *P = pts + (size_t)b * nmax * stride;
     const double *cr = crop_range + ((size_t)b * ncand + pick) * 3;
     int ci = (int)(center_u[(size_t)b * ncand + pick] * (float)n);
     ci = ci < 0 ? 0 : (ci >= n ? n - 1 : ci);
@@ -180,7 +190,7 @@ cuboid_pick_kernel(int nmax, int stride, int ncand, int gmax, int min_points, fl
   for (int q = lane; q < gmax; q += 32) {
     bool keep = q < ng;
     if (keep && pick >= 0 && has_boxes) {
-      const float *bx = B + (size_t)q * box_stride;
+      const T *bx = B + (size_t)q * box_stride;
       keep = bx[0] >= st[1] && bx[1] >= st[2] && bx[2] >= st[3] && bx[0] <= st[4] && bx[1] <= st[5] && bx[2] <= st[6];
     }
     box_keep[(size_t)b * gmax + q] = keep ? 1 : 0;
@@ -189,13 +199,14 @@ cuboid_pick_kernel(int nmax, int stride, int ncand, int gmax, int min_points, fl
 
 // ------------------------------------------------------------------ compaction + sampling
 // order-preserving list of the points inside crop[b]: one CTA per scene, block scan per 1024-point chunk
+template <typename T>
 __global__ void __launch_bounds__(1024)
-compact_kernel(int nmax, int stride, const int *__restrict__ npts, const float *__restrict__ pts,
+compact_kernel(int nmax, int stride, const int *__restrict__ npts, const T *__restrict__ pts,
                const double *__restrict__ crop, int *__restrict__ list, int *__restrict__ count) {
   __shared__ int warp_sum[32];
   __shared__ int base;
   const int b = blockIdx.x, n = min(npts[b], nmax), lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const float *P = pts + (size_t)b * nmax * stride;
+  const T *P = pts + (size_t)b * nmax * stride;
   const double *cb = crop + b * 6;
   if (threadIdx.x == 0) base = 0;
   __syncthreads();
@@ -203,7 +214,7 @@ compact_kernel(int nmax, int stride, const int *__restrict__ npts, const float *
     const int i = i0 + threadIdx.x;
     bool in = false;
     if (i < n) {
-      const float x = P[(size_t)i * stride], y = P[(size_t)i * stride + 1], z = P[(size_t)i * stride + 2];
+      const T x = P[(size_t)i * stride], y = P[(size_t)i * stride + 1], z = P[(size_t)i * stride + 2];
       in = (double)x <= cb[3] && (double)y <= cb[4] && (double)z <= cb[5] && (double)x >= cb[0] && (double)y >= cb[1] &&
            (double)z >= cb[2];
     }
@@ -244,11 +255,11 @@ __device__ __forceinline__ uint32_t feistel(uint32_t x, int half_bits, uint32_t 
 // kEx (the ScanNet item, datasets/scannet_anonymous_aligned_image.py:507-532) also writes list_pos = perm_b(i), the
 // position in the cropped cloud, and rgb_out[b][i] = the first rgb_stride columns of the RAW scene's row list_pos --
 // the reference indexes the uncropped scene with the cropped cloud's choices.
-template <bool kEx>
+template <typename T, bool kEx>
 __global__ void __launch_bounds__(256)
-sample_kernel(int nmax, int stride, int nsample, const float *__restrict__ pts, const int *__restrict__ list,
-              const int *__restrict__ count, const uint32_t *__restrict__ seed, float *__restrict__ out,
-              int *__restrict__ choice, int rgb_stride, int *__restrict__ list_pos, float *__restrict__ rgb_out) {
+sample_kernel(int nmax, int stride, int nsample, const T *__restrict__ pts, const int *__restrict__ list,
+              const int *__restrict__ count, const uint32_t *__restrict__ seed, T *__restrict__ out,
+              int *__restrict__ choice, int rgb_stride, int *__restrict__ list_pos, T *__restrict__ rgb_out) {
   const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nsample) return;
   const int m = count[b];
@@ -266,14 +277,14 @@ sample_kernel(int nmax, int stride, int nsample, const float *__restrict__ pts, 
     }
     src = list[(size_t)b * nmax + j];
   }
-  const float *p = pts + ((size_t)b * nmax + src) * stride;
-  float *o = out + ((size_t)b * nsample + i) * stride;
-  for (int c = 0; c < stride; ++c) o[c] = m > 0 ? p[c] : 0.f;
+  const T *p = pts + ((size_t)b * nmax + src) * stride;
+  T *o = out + ((size_t)b * nsample + i) * stride;
+  for (int c = 0; c < stride; ++c) o[c] = m > 0 ? p[c] : (T)0;
   choice[(size_t)b * nsample + i] = m > 0 ? src : -1;
   if (kEx) {
-    const float *q = pts + ((size_t)b * nmax + j) * stride;
-    float *r = rgb_out + ((size_t)b * nsample + i) * rgb_stride;
-    for (int c = 0; c < rgb_stride; ++c) r[c] = m > 0 ? q[c] : 0.f;
+    const T *q = pts + ((size_t)b * nmax + j) * stride;
+    T *r = rgb_out + ((size_t)b * nsample + i) * rgb_stride;
+    for (int c = 0; c < rgb_stride; ++c) r[c] = m > 0 ? q[c] : (T)0;
     list_pos[(size_t)b * nsample + i] = m > 0 ? (int)j : -1;
   }
 }
@@ -282,56 +293,59 @@ sample_kernel(int nmax, int stride, int nsample, const float *__restrict__ pts, 
 // datasets/scannet_anonymous_aligned_image.py:545-604 on float32 rows: x <- -x (YZ flip), y <- -y (XZ flip), exact;
 // then np.dot(pc[:, 0:3], rot^T) with a float64 rot -- numpy promotes to float64 and BLAS accumulates the three
 // products with fused multiply-adds, the result is stored back as float32 -- and finally `pc[:, 0:3] *= scale`
-// with a float64 scale: float64 product, stored as float32.
+// with a float64 scale: float64 product, stored as float32.  On float64 rows (SUN RGB-D's scene files,
+// datasets/sunrgbd_anonymous_aligned_image.py:664-709) the same statements run in float64 end to end: the same fused
+// chain, no rounding between the rotation and the scale.  The flips are exact in both types.
+template <typename T>
 __global__ void __launch_bounds__(256)
 flip2_rotate_scale_kernel(int nmax, int stride, const int *__restrict__ npts, const float *__restrict__ flip_yz,
                           const float *__restrict__ flip_xz, const double *__restrict__ rot,
-                          const double *__restrict__ scale, float *__restrict__ pts) {
+                          const double *__restrict__ scale, T *__restrict__ pts) {
   const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nmax || (npts && i >= npts[b])) return;
-  float *p = pts + ((size_t)b * nmax + i) * stride;
+  T *p = pts + ((size_t)b * nmax + i) * stride;
   const double *R = rot + b * 9;
-  const double x = (double)__fmul_rn(p[0], flip_yz[b]), y = (double)__fmul_rn(p[1], flip_xz[b]), z = (double)p[2];
+  const double x = (double)(p[0] * (T)flip_yz[b]), y = (double)(p[1] * (T)flip_xz[b]), z = (double)p[2];
   const double s = scale[b];
-  float v[3];
+  T v[3];
 #pragma unroll
   for (int j = 0; j < 3; ++j)
-    v[j] = __double2float_rn(__fma_rn(z, R[j * 3 + 2], __fma_rn(y, R[j * 3 + 1], __dmul_rn(x, R[j * 3]))));
+    v[j] = from_double<T>(__fma_rn(z, R[j * 3 + 2], __fma_rn(y, R[j * 3 + 1], __dmul_rn(x, R[j * 3]))));
 #pragma unroll
-  for (int j = 0; j < 3; ++j) p[j] = __double2float_rn(__dmul_rn((double)v[j], s));
+  for (int j = 0; j < 3; ++j) p[j] = from_double<T>(__dmul_rn((double)v[j], s));
 }
 
 // per-scene extent of the first three columns: dims (b, 6) = min xyz | max xyz
+template <typename T>
 __global__ void __launch_bounds__(256)
-extent_kernel(int nmax, int stride, const int *__restrict__ npts, const float *__restrict__ pts,
-              float *__restrict__ dims) {
+extent_kernel(int nmax, int stride, const int *__restrict__ npts, const T *__restrict__ pts, T *__restrict__ dims) {
   const int b = blockIdx.x;
   const int n = npts ? min(npts[b], nmax) : nmax;
-  const float *P = pts + (size_t)b * nmax * stride;
-  float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
+  const T *P = pts + (size_t)b * nmax * stride;
+  T mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
-      const float v = P[(size_t)i * stride + a];
-      mn[a] = fminf(mn[a], v);
-      mx[a] = fmaxf(mx[a], v);
+      const T v = P[(size_t)i * stride + a];
+      mn[a] = vmin(mn[a], v);
+      mx[a] = vmax(mx[a], v);
     }
   }
-  __shared__ float s_mn[8][3], s_mx[8][3];
+  __shared__ T s_mn[8][3], s_mx[8][3];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1)
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
-      mn[a] = fminf(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
-      mx[a] = fmaxf(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
+      mn[a] = vmin(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
+      mx[a] = vmax(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
     }
   const int w = threadIdx.x >> 5;
   if ((threadIdx.x & 31) == 0)
     for (int a = 0; a < 3; ++a) { s_mn[w][a] = mn[a]; s_mx[w][a] = mx[a]; }
   __syncthreads();
   if (threadIdx.x < 3) {
-    float lo = s_mn[0][threadIdx.x], hi = s_mx[0][threadIdx.x];
-    for (int q = 1; q < (int)(blockDim.x >> 5); ++q) { lo = fminf(lo, s_mn[q][threadIdx.x]); hi = fmaxf(hi, s_mx[q][threadIdx.x]); }
+    T lo = s_mn[0][threadIdx.x], hi = s_mx[0][threadIdx.x];
+    for (int q = 1; q < (int)(blockDim.x >> 5); ++q) { lo = vmin(lo, s_mn[q][threadIdx.x]); hi = vmax(hi, s_mx[q][threadIdx.x]); }
     dims[b * 6 + threadIdx.x] = lo;
     dims[b * 6 + 3 + threadIdx.x] = hi;
   }
@@ -364,6 +378,62 @@ image_augment_kernel(int h, int w, const unsigned char *__restrict__ in, const u
   }
 }
 
+// ------------------------------------------------------------------ host launchers shared by the fp32 / fp64 entry points
+template <typename T>
+int random_cuboid(int b, int nmax, int stride, int ncand, int gmax, int box_stride, int min_points, float aspect_min,
+                  const int *npts, const T *points, const T *range_xyz, const double *crop_range, const float *center_u,
+                  const T *boxes, const int *nbox, T *stats_scratch, int *chosen, double *crop,
+                  unsigned char *box_keep, void *stream) {
+  if (b < 0 || nmax <= 0 || stride < 3 || ncand <= 0 || gmax < 0 || box_stride < 3) return CODA_EINVAL;
+  if (b == 0) return CODA_OK;
+  if (!npts || !points || !range_xyz || !crop_range || !center_u || !nbox || !stats_scratch || !chosen || !crop ||
+      (gmax > 0 && (!boxes || !box_keep)) || b > 65535)
+    return CODA_EINVAL;
+  cudaStream_t s = (cudaStream_t)stream;
+  cuboid_stats_kernel<T><<<dim3(ncand, b), 256, 0, s>>>(nmax, stride, ncand, npts, points, range_xyz, crop_range,
+                                                        center_u, stats_scratch);
+  cuboid_pick_kernel<T><<<b, 32, 0, s>>>(nmax, stride, ncand, gmax, min_points, aspect_min, npts, points, range_xyz,
+                                         crop_range, center_u, stats_scratch, boxes, box_stride, nbox, chosen, crop,
+                                         box_keep);
+  return launch_status();
+}
+
+template <typename T>
+int sample_points(int b, int nmax, int stride, int nsample, const int *npts, const T *points, const double *crop,
+                  const unsigned int *seed, int *list_scratch, int *count, T *out, int *choice, T *dims,
+                  void *stream) {
+  if (b < 0 || nmax <= 0 || stride < 3 || nsample <= 0) return CODA_EINVAL;
+  if (b == 0) return CODA_OK;
+  if (!npts || !points || !crop || !seed || !list_scratch || !count || !out || !choice || !dims || b > 65535)
+    return CODA_EINVAL;
+  cudaStream_t s = (cudaStream_t)stream;
+  compact_kernel<T><<<b, 1024, 0, s>>>(nmax, stride, npts, points, crop, list_scratch, count);
+  sample_kernel<T, false><<<dim3((nsample + 255) / 256, b), 256, 0, s>>>(nmax, stride, nsample, points, list_scratch,
+                                                                         count, seed, out, choice, 0, nullptr, nullptr);
+  extent_kernel<T><<<b, 256, 0, s>>>(nsample, stride, nullptr, out, dims);
+  return launch_status();
+}
+
+template <typename T>
+int flip2_rotate_scale(int b, int nmax, int stride, const int *npts, const float *flip_yz, const float *flip_xz,
+                       const double *rot, const double *scale, T *points, void *stream) {
+  if (b < 0 || nmax < 0 || stride < 3) return CODA_EINVAL;
+  if (b == 0 || nmax == 0) return CODA_OK;
+  if (!flip_yz || !flip_xz || !rot || !scale || !points || b > 65535) return CODA_EINVAL;
+  flip2_rotate_scale_kernel<T><<<dim3((nmax + 255) / 256, b), 256, 0, (cudaStream_t)stream>>>(
+      nmax, stride, npts, flip_yz, flip_xz, rot, scale, points);
+  return launch_status();
+}
+
+template <typename T>
+int points_extent(int b, int nmax, int stride, const int *npts, const T *points, T *dims, void *stream) {
+  if (b < 0 || nmax <= 0 || stride < 3) return CODA_EINVAL;
+  if (b == 0) return CODA_OK;
+  if (!points || !dims) return CODA_EINVAL;
+  extent_kernel<T><<<b, 256, 0, (cudaStream_t)stream>>>(nmax, stride, npts, points, dims);
+  return launch_status();
+}
+
 }  // namespace
 
 extern "C" {
@@ -382,33 +452,31 @@ int coda_random_cuboid(int b, int nmax, int stride, int ncand, int gmax, int box
                        float aspect_min, const int *npts, const float *points, const float *range_xyz,
                        const double *crop_range, const float *center_u, const float *boxes, const int *nbox,
                        float *stats_scratch, int *chosen, double *crop, unsigned char *box_keep, void *stream) {
-  if (b < 0 || nmax <= 0 || stride < 3 || ncand <= 0 || gmax < 0 || box_stride < 3) return CODA_EINVAL;
-  if (b == 0) return CODA_OK;
-  if (!npts || !points || !range_xyz || !crop_range || !center_u || !nbox || !stats_scratch || !chosen || !crop ||
-      (gmax > 0 && (!boxes || !box_keep)) || b > 65535)
-    return CODA_EINVAL;
-  cudaStream_t s = (cudaStream_t)stream;
-  cuboid_stats_kernel<<<dim3(ncand, b), 256, 0, s>>>(nmax, stride, ncand, npts, points, range_xyz, crop_range, center_u,
-                                                     stats_scratch);
-  cuboid_pick_kernel<<<b, 32, 0, s>>>(nmax, stride, ncand, gmax, min_points, aspect_min, npts, points, range_xyz,
-                                      crop_range, center_u, stats_scratch, boxes, box_stride, nbox, chosen, crop,
-                                      box_keep);
-  return launch_status();
+  return random_cuboid<float>(b, nmax, stride, ncand, gmax, box_stride, min_points, aspect_min, npts, points, range_xyz,
+                              crop_range, center_u, boxes, nbox, stats_scratch, chosen, crop, box_keep, stream);
+}
+
+int coda_random_cuboid_f64(int b, int nmax, int stride, int ncand, int gmax, int box_stride, int min_points,
+                           float aspect_min, const int *npts, const double *points, const double *range_xyz,
+                           const double *crop_range, const float *center_u, const double *boxes, const int *nbox,
+                           double *stats_scratch, int *chosen, double *crop, unsigned char *box_keep, void *stream) {
+  return random_cuboid<double>(b, nmax, stride, ncand, gmax, box_stride, min_points, aspect_min, npts, points,
+                               range_xyz, crop_range, center_u, boxes, nbox, stats_scratch, chosen, crop, box_keep,
+                               stream);
 }
 
 int coda_sample_points(int b, int nmax, int stride, int nsample, const int *npts, const float *points,
                        const double *crop, const unsigned int *seed, int *list_scratch, int *count, float *out,
                        int *choice, float *dims, void *stream) {
-  if (b < 0 || nmax <= 0 || stride < 3 || nsample <= 0) return CODA_EINVAL;
-  if (b == 0) return CODA_OK;
-  if (!npts || !points || !crop || !seed || !list_scratch || !count || !out || !choice || !dims || b > 65535)
-    return CODA_EINVAL;
-  cudaStream_t s = (cudaStream_t)stream;
-  compact_kernel<<<b, 1024, 0, s>>>(nmax, stride, npts, points, crop, list_scratch, count);
-  sample_kernel<false><<<dim3((nsample + 255) / 256, b), 256, 0, s>>>(nmax, stride, nsample, points, list_scratch,
-                                                                      count, seed, out, choice, 0, nullptr, nullptr);
-  extent_kernel<<<b, 256, 0, s>>>(nsample, stride, nullptr, out, dims);
-  return launch_status();
+  return sample_points<float>(b, nmax, stride, nsample, npts, points, crop, seed, list_scratch, count, out, choice,
+                              dims, stream);
+}
+
+int coda_sample_points_f64(int b, int nmax, int stride, int nsample, const int *npts, const double *points,
+                           const double *crop, const unsigned int *seed, int *list_scratch, int *count, double *out,
+                           int *choice, double *dims, void *stream) {
+  return sample_points<double>(b, nmax, stride, nsample, npts, points, crop, seed, list_scratch, count, out, choice,
+                               dims, stream);
 }
 
 int coda_sample_points_ex(int b, int nmax, int stride, int nsample, int rgb_stride, const int *npts,
@@ -421,31 +489,33 @@ int coda_sample_points_ex(int b, int nmax, int stride, int nsample, int rgb_stri
       (rgb_stride > 0 && !rgb_out) || b > 65535)
     return CODA_EINVAL;
   cudaStream_t s = (cudaStream_t)stream;
-  compact_kernel<<<b, 1024, 0, s>>>(nmax, stride, npts, points, crop, list_scratch, count);
-  sample_kernel<true><<<dim3((nsample + 255) / 256, b), 256, 0, s>>>(nmax, stride, nsample, points, list_scratch,
-                                                                     count, seed, out, choice, rgb_stride, list_pos,
-                                                                     rgb_out);
-  extent_kernel<<<b, 256, 0, s>>>(nsample, stride, nullptr, out, dims);
+  compact_kernel<float><<<b, 1024, 0, s>>>(nmax, stride, npts, points, crop, list_scratch, count);
+  sample_kernel<float, true><<<dim3((nsample + 255) / 256, b), 256, 0, s>>>(nmax, stride, nsample, points,
+                                                                            list_scratch, count, seed, out, choice,
+                                                                            rgb_stride, list_pos, rgb_out);
+  extent_kernel<float><<<b, 256, 0, s>>>(nsample, stride, nullptr, out, dims);
   return launch_status();
 }
 
 int coda_points_flip2_rotate_scale(int b, int nmax, int stride, const int *npts, const float *flip_yz,
                                    const float *flip_xz, const double *rot, const double *scale, float *points,
                                    void *stream) {
-  if (b < 0 || nmax < 0 || stride < 3) return CODA_EINVAL;
-  if (b == 0 || nmax == 0) return CODA_OK;
-  if (!flip_yz || !flip_xz || !rot || !scale || !points || b > 65535) return CODA_EINVAL;
-  flip2_rotate_scale_kernel<<<dim3((nmax + 255) / 256, b), 256, 0, (cudaStream_t)stream>>>(
-      nmax, stride, npts, flip_yz, flip_xz, rot, scale, points);
-  return launch_status();
+  return flip2_rotate_scale<float>(b, nmax, stride, npts, flip_yz, flip_xz, rot, scale, points, stream);
+}
+
+int coda_points_flip2_rotate_scale_f64(int b, int nmax, int stride, const int *npts, const float *flip_yz,
+                                       const float *flip_xz, const double *rot, const double *scale, double *points,
+                                       void *stream) {
+  return flip2_rotate_scale<double>(b, nmax, stride, npts, flip_yz, flip_xz, rot, scale, points, stream);
 }
 
 int coda_points_extent(int b, int nmax, int stride, const int *npts, const float *points, float *dims, void *stream) {
-  if (b < 0 || nmax <= 0 || stride < 3) return CODA_EINVAL;
-  if (b == 0) return CODA_OK;
-  if (!points || !dims) return CODA_EINVAL;
-  extent_kernel<<<b, 256, 0, (cudaStream_t)stream>>>(nmax, stride, npts, points, dims);
-  return launch_status();
+  return points_extent<float>(b, nmax, stride, npts, points, dims, stream);
+}
+
+int coda_points_extent_f64(int b, int nmax, int stride, const int *npts, const double *points, double *dims,
+                           void *stream) {
+  return points_extent<double>(b, nmax, stride, npts, points, dims, stream);
 }
 
 int coda_image_augment(int b, int h, int w, const unsigned char *in, const unsigned char *flip, const float *gain,

@@ -7,6 +7,11 @@
  * coda_pointnet2.h.  Scenes are padded: points (b, nmax, stride) fp32 with npts (b) valid rows (columns 0-2 = xyz,
  * the others -- colour, height -- travel along); boxes (b, gmax, box_stride) fp32 rows [cx, cy, cz, ...] with
  * nbox (b) valid rows.  All randomness comes in as small device arrays drawn by the caller.
+ *
+ * The `_f64` entry points are the same kernels on float64 points and boxes (dims, stats and samples in float64 too),
+ * for SUN RGB-D, whose `_pc.npz` / `_bbox.npy` arrays are float64: there the reference's flip, rotation, scale,
+ * RandomCuboid and sampling all run in float64 (datasets/sunrgbd_anonymous_aligned_image.py:660-771).  The float32
+ * entry points are unchanged by them.
  */
 #ifndef CODA_DATA_H
 #define CODA_DATA_H
@@ -28,6 +33,10 @@ int coda_scene_transform(int b, int nmax, int stride, const int *npts, const flo
 /* dims (b, 6) = [min xyz | max xyz] of the valid points (npts may be NULL: all nmax rows). */
 int coda_points_extent(int b, int nmax, int stride, const int *npts, const float *points, float *dims, void *stream);
 
+/* float64 twin: replaces RandomCuboid's range_xyz (random_cuboid.py:39-41) on the float64 SUN RGB-D cloud. */
+int coda_points_extent_f64(int b, int nmax, int stride, const int *npts, const double *points, double *dims,
+                           void *stream);
+
 /*
  * RandomCuboid (utils/random_cuboid.py:39-116) with all `ncand` attempts of a scene evaluated at once.
  *   range_xyz (b, 3) = extent of the cloud; crop_range (b, ncand, 3) fp64 in [min_crop, max_crop] (the reference's
@@ -43,6 +52,16 @@ int coda_random_cuboid(int b, int nmax, int stride, int ncand, int gmax, int box
                        float *stats_scratch, int *chosen, double *crop, unsigned char *box_keep, void *stream);
 
 /*
+ * float64 twin (points, range_xyz, boxes, stats_scratch in float64): replaces the SUN RGB-D item's RandomCuboid call
+ *   (datasets/sunrgbd_anonymous_aligned_image.py:714-717) on its float64 cloud and boxes; `target_boxes.sum() > 0` is
+ *   summed in float64.
+ */
+int coda_random_cuboid_f64(int b, int nmax, int stride, int ncand, int gmax, int box_stride, int min_points,
+                           float aspect_min, const int *npts, const double *points, const double *range_xyz,
+                           const double *crop_range, const float *center_u, const double *boxes, const int *nbox,
+                           double *stats_scratch, int *chosen, double *crop, unsigned char *box_keep, void *stream);
+
+/*
  * pc_util.random_sampling (:24-32) of the points inside crop (b, 6): out (b, nsample, stride), choice (b, nsample)
  *   = row of the raw scene each sample came from, count (b) = points inside, dims (b, 6) = extent of the sample
  *   (point_cloud_dims_min / max, :748-749).  Without replacement when count >= nsample (a keyed Feistel permutation
@@ -51,6 +70,14 @@ int coda_random_cuboid(int b, int nmax, int stride, int ncand, int gmax, int box
 int coda_sample_points(int b, int nmax, int stride, int nsample, const int *npts, const float *points,
                        const double *crop, const unsigned int *seed, int *list_scratch, int *count, float *out,
                        int *choice, float *dims, void *stream);
+
+/*
+ * float64 twin (points, out, dims in float64), same sampler and same positions: replaces the SUN RGB-D item's
+ *   random_sampling and point_cloud_dims_min / max (:763-771), which stay float64 there.
+ */
+int coda_sample_points_f64(int b, int nmax, int stride, int nsample, const int *npts, const double *points,
+                           const double *crop, const unsigned int *seed, int *list_scratch, int *count, double *out,
+                           int *choice, double *dims, void *stream);
 
 /*
  * coda_sample_points plus the ScanNet item's gathers (datasets/scannet_anonymous_aligned_image.py:507-532), in the same
@@ -76,6 +103,16 @@ int coda_sample_points_ex(int b, int nmax, int stride, int nsample, int rgb_stri
 int coda_points_flip2_rotate_scale(int b, int nmax, int stride, const int *npts, const float *flip_yz,
                                    const float *flip_xz, const double *rot, const double *scale, float *points,
                                    void *stream);
+
+/*
+ * float64 twin on (b, nmax, stride) fp64 rows: the same fused chain with no rounding to float32 anywhere.  Replaces the
+ *   SUN RGB-D item's flip about YZ, np.dot with rotz and float64 scale (:664-709, flip_xz = +1) on the whole raw
+ *   scene and on the boxes' centres, and the np.dot(rotz(-heading), corners) of my_compute_box_3d (:288-298; one
+ *   "scene" per box, 8 rows, scale 1).
+ */
+int coda_points_flip2_rotate_scale_f64(int b, int nmax, int stride, const int *npts, const float *flip_yz,
+                                       const float *flip_xz, const double *rot, const double *scale, double *points,
+                                       void *stream);
 
 /*
  * Image augmentation of :624-655 on uint8 HWC images: horizontal flip (flip (b) != 0), per-channel gain (b, 3) and
